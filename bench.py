@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""Headline benchmark of the B200 HSTU hot path (contract: see the task statement / DESIGN.md section "Measurement").
+"""Headline benchmark of the H100 HSTU hot path (DESIGN.md section "Measurement").
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload hstu_large|attn]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|triton] [--workload hstu_large|attn] [--dump-outputs DIR]
 
 Workload `hstu_large` (default; BASELINE.json metric "user-seqs/sec HSTU-large L=8192 d=256 bf16"):
   a 16-layer STU stack, D=256, H=8, dqk=dv=32, bf16, over a synthetic jagged batch of `--batch` user sequences per GPU
@@ -11,10 +11,14 @@ Workload `hstu_large` (default; BASELINE.json metric "user-seqs/sec HSTU-large L
 Workload `attn`: the reference microbench (B=512, H=4, d in {64,128}, fwd+bwd of hstu_mha only).
 
 `--impl triton` (workload attn only) times the reference's own Triton kernel (`triton_hstu_mha`, sort_by_length=True,
-enable_tma=False, autotuned; fetched into the git-ignored baseline/_ref/ by scripts/fetch_triton_baseline.py) on the same
-seeded inputs with the same CUDA-event method: the GPU comparator the north-star names.
+enable_tma=False, autotuned; copied into the git-ignored oracle/_ref/ by oracle/fetch_reference_eager.py) on the same
+seeded inputs with the same CUDA-event method.
+
 `--impl reference` times the CPU port of the reference eager path (oracle/) on the host cores on a bounded sample of
-the same workload (the Python reference itself cannot travel to the GPU box).  Rank 0 only.
+the same workload.  Rank 0 only.
+`--dump-outputs DIR` (our arm, rank 0) writes what the last timed step computed -- the arrays its caller receives -- as
+DIR/<name>.npy in float32 / float64 (64 MB at most: large arrays are a fixed, seeded sample of their rows or elements).  The
+inputs depend only on the arguments, so two builds of the project can be compared output for output.
 """
 import argparse
 import json
@@ -43,12 +47,16 @@ def parse_args():
     ap.add_argument("--layers", type=int, default=16)
     ap.add_argument("--attn-dim", type=int, default=128, help="head dim of the attn microbench workload")
     ap.add_argument("--attn-heads", type=int, default=4)
-    ap.add_argument("--attn-impl", type=int, default=0, help="0 auto, 1 generic kernels, 2 force tcgen05")
+    ap.add_argument("--attn-impl", type=int, default=0, help="0 auto, 1 generic kernels, 2 force wgmma")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
-                    help="weak: --batch sequences per GPU (default, what the driver's scaling run measures); strong: --batch "
+                    help="weak: --batch sequences per GPU (default); strong: --batch "
                          "sequences in total, sharded over the ranks balanced by sum(len^2) (distributed.shard_sequences)")
-    return ap.parse_args()
+    a = ap.parse_args()
+    if a.dump_outputs and a.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of our arm; it is not available with --impl " + a.impl)
+    return a
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -60,20 +68,49 @@ def measured_peaks():
         d = json.load(open(path))
         return dict(hbm_gbs=d["hbm_gbs"], tflops_burst=d["bf16_tflops"], tflops_sustained=d["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- a ceiling, not a measured rate
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source="H100 SXM data sheet (not measured)")
 
 
-def ncu_traffic(cfg):
-    """DRAM bytes per launch of the attention backward kernel from the committed `ncu --set full` capture
-    (profiles/ncu_traffic.json, written by scripts/ncu_traffic.py) -- only if it was taken on this attention shape."""
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        d = json.load(open(path))
-        if d.get("attn_shape") == cfg.get("attn_shape"):
-            return d["kernels"]["attn_bwd"]["dram_bytes"], f"profiles/ncu_traffic.json ({d['source']}; {d['workload']})"
-    except Exception:
-        pass
-    return None, None
+_DUMP_BYTES = 64_000_000  # 64 MB
+
+
+def dump_outputs(path, arrays):
+    """arrays: name -> tensor.  Saved as float32 (float64 for 0-d / 1-element results); arrays beyond their share of the 64 MB
+    budget are reduced to a fixed, seeded sample of rows (2-D and more) or elements, whose indices are saved next to them."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    g = torch.Generator().manual_seed(20260)
+    budget = _DUMP_BYTES - 512 * 2 * len(arrays)  # .npy headers of the outputs and of the row indices
+    items = sorted(arrays.items(), key=lambda kv: kv[1].numel())  # small arrays whole; the rest share what is left
+    for i, (name, t) in enumerate(items):
+        t = t.detach().float().cpu()
+        if t.numel() <= 1:
+            np.save(os.path.join(path, f"{name}.npy"), t.double().numpy())
+            budget -= 8
+            continue
+        share = budget // (len(items) - i)
+        row_bytes = (t.numel() // t.shape[0]) * 4
+        if t.numel() * 4 > share:
+            n = max(1, share // (row_bytes + 8))
+            idx = torch.randperm(t.shape[0], generator=g)[:n].sort().values
+            np.save(os.path.join(path, f"{name}.rows.npy"), idx.numpy())
+            t = t[idx]
+            budget -= n * 8
+        np.save(os.path.join(path, f"{name}.npy"), t.numpy())
+        budget -= t.numel() * 4
+
+
+def ensure_built():
+    """Build the library if it is missing.  A tree that build() has left is used as it is: it may be read-only, so nothing
+    is recompiled into it at run time."""
+    from generative_recommenders_b200 import _lib
+    from generative_recommenders_b200.build import build
+
+    if not os.path.exists(_lib.LIB_PATH):
+        build()
+    _lib.lib()
 
 
 class ClockSampler:
@@ -162,7 +199,6 @@ def attn_bytes(lengths, heads, dqk, dv, elt=2):
 def run_ours(args):
     import torch.distributed as dist
     from generative_recommenders_b200 import _lib
-    from generative_recommenders_b200.build import build
     from generative_recommenders_b200.modules.stu import STULayer, STULayerConfig, STUStack
     from generative_recommenders_b200.ops.hstu_attention import hstu_mha
 
@@ -173,12 +209,10 @@ def run_ours(args):
         raise SystemExit("bench.py needs a CUDA device: the product path has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
-    if rank == 0:
-        build()
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
         dist.barrier()
-    _lib.lib()
+    ensure_built()
     D, H, dh, layers = 256, 8, 32, args.layers
     # the same seeded lengths on every rank (weak scaling: identical sum of len^2 per GPU, so the curve measures the collective
     # and not a straggler); the activations / gradients differ per rank (seeded below)
@@ -197,6 +231,7 @@ def run_ours(args):
         seqs_total = args.batch
     L = int(off[-1])
 
+    last = {}  # what the most recent step computed (--dump-outputs)
     if args.workload == "hstu_large":
         torch.manual_seed(7)  # identical initial weights on every rank (DDP broadcast equivalent)
         stack = STUStack([STULayer(STULayerConfig(embedding_dim=D, num_heads=H, hidden_dim=dh, attention_dim=dh,
@@ -217,6 +252,11 @@ def run_ours(args):
         # is launched on a side stream as soon as that layer's grads are final.  Same code path at N = 1 (no collective).
         reducer = LayerBucketAllReduce(list(stack._stu_layers), world, dev)
 
+        def outputs():
+            out = {"y": last["y"], "loss": last["loss"]}
+            out.update({f"grad.{n}": p.grad for n, p in stack.named_parameters()})
+            return out
+
         def step(e2e: bool):
             if e2e:
                 x = x_host.to(dev, non_blocking=True)
@@ -227,7 +267,9 @@ def run_ours(args):
                 x, o_, n_, l_ = x_dev, off, nt, lengths
             reducer.zero_grad()
             y = stack(x=x, x_lengths=l_, x_offsets=o_, max_seq_len=args.lmax, num_targets=n_)
+            last["y"] = y
             loss = y.float().square().mean()
+            last["loss"] = loss
             loss.backward()
             reducer.wait()
             opt.step()
@@ -241,7 +283,7 @@ def run_ours(args):
                            f"{args.batch} user sequences{'/GPU' if args.scaling == 'weak' else ' in total (sharded by sum len^2)'} (lengths U[0.9,1.0)*Lmax, 1-20 targets, seed 1001 on every rank; activations seeded per rank), dropout 0.2",
                "global_batch": seqs_total, "seq_len": args.lmax, "rows_per_gpu": L,
                "parallelism": f"dp{world} (batch-sharded, per-layer in-place bf16 NCCL all-reduce of the flat gradient bucket overlapped with backward)",
-               "l2": f"inputs + activations per step ({L * D * 2 * 6 / 1e6:.0f} MB+) exceed the 126 MB L2; no explicit flush"}
+               "l2": f"inputs + activations per step ({L * D * 2 * 6 / 1e6:.0f} MB+) exceed the 50 MB L2; no explicit flush"}
         cfg["attn_shape"] = {"batch": args.batch, "lmax": args.lmax, "heads": H, "d": dh}
         aflops = attn_flops(lengths, H, dh, dh)
         abytes = attn_bytes(lengths, H, dh, dh)
@@ -266,16 +308,20 @@ def run_ours(args):
                 q.grad = k.grad = v.grad = None
             o = hstu_mha(args.lmax, alpha, qq, kk, vv, off, num_targets=nt, sort_by_length=True, impl=args.attn_impl)
             o.backward(do)
+            last["o"], last["dq"], last["dk"], last["dv"] = o, qq.grad, kk.grad, vv.grad
             if e2e:
                 return float(o[0, 0, 0].item())
             return o
+
+        def outputs():
+            return {"out": last["o"], "dq": last["dq"], "dk": last["dk"], "dv": last["dv"]}
 
         units_per_step = args.batch
         d2h_bytes = 2
         cfg = {"workload": f"hstu_mha fwd+bwd microbench (hstu_attention_bench.py recipe): B={args.batch}, H={Ha}, d={d}, "
                            f"Lmax={args.lmax}, bf16, alpha=1/d, targets<=20", "global_batch": args.batch * world,
                "seq_len": args.lmax, "rows_per_gpu": L, "parallelism": f"dp{world} (independent shards)",
-               "l2": f"q,k,v,o,grads = {L * Ha * d * 2 * 11 / 1e6:.0f} MB per step > 126 MB L2" }
+               "l2": f"q,k,v,o,grads = {L * Ha * d * 2 * 11 / 1e6:.0f} MB per step > 50 MB L2" }
         cfg["attn_shape"] = {"batch": args.batch, "lmax": args.lmax, "heads": Ha, "d": d}
         aflops = attn_flops(lengths, Ha, d, d)
         abytes = attn_bytes(lengths, Ha, d, d)
@@ -314,6 +360,8 @@ def run_ours(args):
         sampler.start()
     ms, launches, events = timed_run(False, args.steps, args.warmup, True)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outputs())
     ms_e2e, _, _ = timed_run(True, args.steps, 1, False)
 
     value = units_per_step * world * args.steps / (ms * 1e-3)
@@ -336,10 +384,10 @@ def run_ours(args):
         tf_b = aflops["bwd"] / (kt["attn_bwd"] * 1e-3) / 1e12
         tf_f = aflops["fwd"] / (kt["attn_fwd"] * 1e-3) / 1e12
         peak = peaks["tflops_sustained"]
-        traffic, traffic_src = ncu_traffic(cfg)
         out["roofline"] = {
             "kernel": "hstu_attn_bwd (dK/dV + dQ kernels of one layer call)", "bound": "tensor", "achieved": tf_b, "peak": peak,
-            "unit": "TFLOP/s", "frac": tf_b / peak, "traffic": traffic, "traffic_source": traffic_src,
+            "unit": "TFLOP/s", "frac": tf_b / peak, "traffic": abytes["bwd"],
+            "traffic_source": "algorithmic bytes per launch (every tensor touched once), not a DRAM measurement",
             "peak_source": peaks["source"] + ", sustained bf16",
             "ms_per_launch": kt["attn_bwd"], "algorithmic_flops_per_launch": aflops["bwd"],
             "fwd": {"achieved": tf_f, "frac": tf_f / peak, "ms_per_launch": kt["attn_fwd"],
@@ -347,9 +395,6 @@ def run_ours(args):
                     "hbm_gbs_algorithmic": abytes["fwd"] / (kt["attn_fwd"] * 1e-3) / 1e9},
             "bwd_hbm_gbs_algorithmic": abytes["bwd"] / (kt["attn_bwd"] * 1e-3) / 1e9, "hbm_peak_gbs": peaks["hbm_gbs"],
             "attn_share_of_step": (kt["attn_bwd"] + kt["attn_fwd"]) * per_step_calls / (ms / args.steps),
-            # what bounds the kernel below the tensor peak at this head dim: measured by timing-only ablations, not assumed
-            "bound_evidence": "profiles/r02_ablations.txt (d = 32 backward: tcgen05 issue rate of its N = 32 MMAs, 1464 clk per "
-                              "128 x 128 tile = 0.67 of the bf16 peak for this tiling; forward: serial chain of a TMEM score slot)",
         }
     out["kernel_ms_per_call"] = {k: round(v, 4) for k, v in sorted(kt.items())}
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
@@ -375,7 +420,6 @@ RESEARCH_CFG = {
 
 def run_research(args):
     from generative_recommenders_b200 import _lib
-    from generative_recommenders_b200.build import build
     from generative_recommenders_b200.modules.research_hstu import (RelativeBucketedTimeAndPositionBasedBias,
                                                                     SequentialTransductionUnitJagged)
     from generative_recommenders_b200.modules.sampled_softmax import LocalNegativesSampler, SampledSoftmaxLoss
@@ -383,8 +427,7 @@ def run_research(args):
     c = RESEARCH_CFG[args.workload]
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
-    build()
-    _lib.lib()
+    ensure_built()
     torch.manual_seed(7)
     D, H, d, n, B, R, V = c["D"], c["H"], c["d"], c["n"], c["B"], c["R"], c["V"]
     emb = torch.nn.Embedding(V, D)
@@ -411,6 +454,8 @@ def run_research(args):
     nxt = torch.arange(1, L + 1, device=dev).clamp(max=L - 1)  # next-item supervision inside the flat row order (synthetic)
     w_dev = torch.ones(L, device=dev, dtype=torch.bfloat16)
 
+    last = {}  # what the most recent step computed (--dump-outputs)
+
     def step(e2e):
         ids = ids_host.to(dev, non_blocking=True) if e2e else ids_dev
         ts = ts_host.to(dev, non_blocking=True) if e2e else ts_dev
@@ -423,6 +468,7 @@ def run_research(args):
                                           supervision_weights=w_dev, negatives_sampler=sampler)
         loss.backward()
         opt.step()
+        last["loss"] = loss
         return float(loss.item()) if e2e else loss
 
     def timed(e2e, steps, warmup, with_events):
@@ -445,6 +491,9 @@ def run_research(args):
     sampler_c.start()
     ms, launches, events = timed(False, args.steps, args.warmup, True)
     clocks = sampler_c.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"loss": last["loss"], **{f"grad.{n}": p.grad for n, p in model.named_parameters()
+                                                                  if p.grad is not None}})
     ms_e2e, _, _ = timed(True, args.steps, 1, False)
     kt = {k: round(sum(a.elapsed_time(b) for a, b in v) / max(1, len(v)), 4) for k, v in (events or {}).items()}
     print(json.dumps({
@@ -454,22 +503,22 @@ def run_research(args):
         "config": {"workload": f"{c['name']}: item embedding ({V} x {D}) -> {c['layers']} research HSTU blocks (D={D}, H={H}, dqk=dv={d}, "
                                f"n={n}, relative position + time bias) -> sampled softmax ({R} negatives, l2 norm, T=0.05), batch {B}, "
                                f"{L} rows, dropout 0.2, bf16", "global_batch": B, "seq_len": n, "rows_per_gpu": L,
-                   "l2": "the whole working set fits the 126 MB L2 except the embedding table; launch-bound at this size"},
+                   "l2": "the whole working set fits the 50 MB L2 except the embedding table; launch-bound at this size"},
         "e2e": {"value": B * args.steps / (ms_e2e * 1e-3), "unit": "sequences/s", "h2d_bytes_per_step": ids_host.numel() * 8 + ts_host.numel() * 8,
                 "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": launches, "clocks": clocks, "kernel_ms_per_call": kt}))
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# GPU comparator: the reference's own Triton kernel (unmodified, from baseline/_ref) on the same inputs
+# GPU comparator: the reference's own Triton kernel (unmodified, from oracle/_ref) on the same inputs
 # ----------------------------------------------------------------------------------------------------------------
 def run_triton(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    ref_root = os.path.join(ROOT, "baseline", "_ref")
+    ref_root = os.path.join(ROOT, "oracle", "_ref")
     if args.workload != "attn" or not os.path.isdir(os.path.join(ref_root, "generative_recommenders")):
-        print(json.dumps({"impl": "triton", "unavailable": "needs --workload attn and baseline/_ref (scripts/fetch_triton_baseline.py)"}))
+        print(json.dumps({"impl": "triton", "unavailable": "needs --workload attn and oracle/_ref (oracle/fetch_reference_eager.py)"}))
         return
     sys.path.insert(0, ref_root)
     try:
@@ -568,7 +617,7 @@ _REF_LAYER = None
 
 def reference_layer():
     """The reference's OWN eager STULayer (unmodified Python, fetched into the git-ignored oracle/_ref/ by
-    scripts/fetch_reference_eager.py; fbgemm_gpu's three jagged ops come from oracle/fbgemm_shim.py), HammerKernel.PYTORCH, fp32.
+    oracle/fetch_reference_eager.py; fbgemm_gpu's three jagged ops come from oracle/fbgemm_shim.py), HammerKernel.PYTORCH, fp32.
     None if oracle/_ref is absent (then the oracle port is timed instead)."""
     global _REF_LAYER
     if _REF_LAYER is None:

@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# HSTU_B200_LIB: another build of the same ABI (compile-time variants for A/B measurements, scripts/build_variant.py)
+# HSTU_B200_LIB: another build of the same ABI (compile-time variants for A/B measurements: HSTU_EXP / HSTU_EXP_SRC of build.py)
 LIB_PATH = os.environ.get("HSTU_B200_LIB") or os.path.join(_HERE, "lib", "libhstu_b200.so")
 
 ABI_VERSION = 1
@@ -112,7 +112,7 @@ _selftest: Optional[C.CDLL] = None
 
 
 def selftest_lib() -> C.CDLL:
-    """The TEST library with the tcgen05 / TMA self test (include/hstu_b200_selftest.h); not used by any product code path."""
+    """The TEST library with the wgmma / TMA self test (include/hstu_b200_selftest.h); not used by any product code path."""
     global _selftest
     if _selftest is None:
         path = os.path.join(_HERE, "lib", "libhstu_b200_selftest.so")

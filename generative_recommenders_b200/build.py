@@ -1,13 +1,13 @@
-"""In-tree build of libhstu_b200.so (sm_100a only).
+"""In-tree build of libhstu_b200.so (sm_90a only).
 
     python -m generative_recommenders_b200.build [--force]
 
 Each translation unit under csrc/ is compiled with
-    nvcc -std=c++20 -gencode arch=compute_100a,code=sm_100a -lineinfo -O3
-and linked into generative_recommenders_b200/lib/libhstu_b200.so (+ the test-only libhstu_b200_selftest.so; git-ignored; it travels to the GPU box with the
-repo snapshot).  nvcc cross-compiles without a GPU, so this is also the "does it build" check of __graft_entry__.build().
+    nvcc -std=c++20 -gencode arch=compute_90a,code=sm_90a -lineinfo -O3
+and linked into generative_recommenders_b200/lib/libhstu_b200.so (+ the test-only libhstu_b200_selftest.so; git-ignored).  nvcc cross-compiles without a GPU, so this is also the "does it build" check of __graft_entry__.build().
 """
 import concurrent.futures
+import importlib.util
 import os
 import shutil
 import subprocess
@@ -18,12 +18,12 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(ROOT, "build", "hstu_b200")
 LIB = os.path.join(HERE, "lib", "libhstu_b200.so")
-SELFTEST_LIB = os.path.join(HERE, "lib", "libhstu_b200_selftest.so")  # test infrastructure: tcgen05 / TMA self test + micro-benchmarks
-
-SELFTEST_SOURCES = ["umma_selftest.cu", "tmap.cu"]
-SOURCES = ["api.cu", "attn_generic.cu", "attn_umma_fwd.cu", "attn_umma_bwd.cu", "tmap.cu", "norm.cu", "norm_fast.cu", "jagged.cu", "position.cu", "sampled_softmax.cu", "jagged_bmm.cu"]
+SELFTEST_LIB = os.path.join(HERE, "lib", "libhstu_b200_selftest.so")  # test infrastructure: wgmma / TMA self test
+GEN = os.path.join(OBJ, "gen")  # generated headers (wgmma_ops.cuh, scripts/gen_wgmma_ops.py)
+SELFTEST_SOURCES = ["wgmma_selftest.cu", "tmap.cu"]
+SOURCES = ["api.cu", "attn_generic.cu", "attn_wgmma_fwd.cu", "attn_wgmma_bwd.cu", "tmap.cu", "norm.cu", "norm_fast.cu", "jagged.cu", "position.cu", "sampled_softmax.cu", "jagged_bmm.cu"]
 NVCC_FLAGS = [
-    "-std=c++20", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3",
+    "-std=c++20", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xcudafe", "--diag_suppress=177",
 ]
 
@@ -36,7 +36,8 @@ def _nvcc() -> str:
 
 
 def _deps_mtime() -> float:
-    paths = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "hstu_b200.h"), __file__]
+    paths = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "hstu_b200.h"), __file__,
+                                                                  os.path.join(ROOT, "scripts", "gen_wgmma_ops.py")]
     return max(os.path.getmtime(p) for p in paths)
 
 
@@ -49,11 +50,11 @@ def _compile(src: str, extra, reuse: bool = False) -> str:
     if reuse and os.path.exists(obj):
         return obj
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
-    hdrs.append(os.path.join(ROOT, "include", "hstu_b200.h"))
+    hdrs += [os.path.join(ROOT, "include", "hstu_b200.h"), os.path.join(GEN, "wgmma_ops.cuh")]
     newest = max(os.path.getmtime(p) for p in hdrs + [os.path.join(CSRC, src), __file__])
     if os.path.exists(obj) and os.path.getmtime(obj) >= newest:
         return obj
-    cmd = [_nvcc()] + NVCC_FLAGS + list(extra) + ["-c", os.path.join(CSRC, src), "-o", obj]
+    cmd = [_nvcc()] + NVCC_FLAGS + ["-I", GEN] + list(extra) + ["-c", os.path.join(CSRC, src), "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
@@ -69,7 +70,12 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(os.path.dirname(LIB), exist_ok=True)
     if force and not os.environ.get("HSTU_EXP_SRC"):
         for f in os.listdir(OBJ):
-            os.remove(os.path.join(OBJ, f))
+            if os.path.isfile(os.path.join(OBJ, f)):  # objects only: GEN is a directory, regenerated below
+                os.remove(os.path.join(OBJ, f))
+    spec = importlib.util.spec_from_file_location("gen_wgmma_ops", os.path.join(ROOT, "scripts", "gen_wgmma_ops.py"))
+    gen = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(gen)
+    gen.main(GEN)
     extra = ["-Xptxas", "-v"] if verbose else []
     if os.environ.get("HSTU_DEBUG_SPIN"):
         extra.append("-DHSTU_DEBUG_SPIN")
@@ -87,7 +93,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         objs = dict(zip(all_src, ex.map(lambda s: _compile(s, extra if (not only or s in only) else [], reuse=bool(only) and s not in only),
                                         all_src)))
     for lib, srcs in ((LIB, SOURCES), (SELFTEST_LIB, SELFTEST_SOURCES)):
-        cmd = [_nvcc(), "-shared", "-o", lib] + [objs[s] for s in srcs] + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [_nvcc(), "-shared", "-o", lib] + [objs[s] for s in srcs] + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

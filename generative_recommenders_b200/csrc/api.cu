@@ -1,5 +1,5 @@
 // C-ABI entry points of libhstu_b200.so (declared in include/hstu_b200.h): argument validation, error reporting,
-// dispatch between the tcgen05/TMA kernels and the generic kernels.  No torch / ATen types anywhere.
+// dispatch between the wgmma/TMA kernels and the generic kernels.  No torch / ATen types anywhere.
 #include <stdarg.h>
 #include <string.h>
 
@@ -58,11 +58,11 @@ int bind_device(const void* ptr) {
 }
 
 static int select_impl(const hstu_attn_params* p, bool bwd) {
-  const bool can = umma_supported(*p, bwd);
+  const bool can = wgmma_supported(*p, bwd);
   if (p->impl == HSTU_IMPL_GENERIC) return HSTU_IMPL_GENERIC;
   if (p->impl == HSTU_IMPL_UMMA) {
     if (!can) {
-      set_error("tcgen05 path does not support this problem (dtype=%d dqk=%d dv=%d delta=%d bias=%d)", p->dtype, p->dqk,
+      set_error("wgmma path does not support this problem (dtype=%d dqk=%d dv=%d delta=%d bias=%d)", p->dtype, p->dqk,
                 p->dv, p->delta_q_len, p->pos_w != nullptr || p->ts_w != nullptr);
       return HSTU_ERR_UNSUPPORTED;
     }
@@ -90,7 +90,7 @@ size_t hstu_attn_workspace_bytes(const hstu_attn_params* p, int is_backward) {
   if (validate_attn(p, is_backward != 0) != 0) return 0;
   if (p->batch == 0 || p->total_rows == 0) return 0;
   int impl = select_impl(p, is_backward != 0);
-  if (impl == HSTU_IMPL_UMMA) return umma_workspace_bytes(*p, is_backward != 0);
+  if (impl == HSTU_IMPL_UMMA) return wgmma_workspace_bytes(*p, is_backward != 0);
   return 0;
 }
 
@@ -100,7 +100,7 @@ int hstu_attn_fwd(const hstu_attn_params* p, void* stream) {
   if (int e = bind_device(p->q)) return e;
   int impl = select_impl(p, false);
   if (impl < 0) return impl;
-  if (impl == HSTU_IMPL_UMMA) return attn_umma_fwd(*p, (cudaStream_t)stream);
+  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_fwd(*p, (cudaStream_t)stream);
   return attn_generic_fwd(*p, (cudaStream_t)stream);
 }
 
@@ -110,7 +110,7 @@ int hstu_attn_bwd(const hstu_attn_params* p, void* stream) {
   if (int e = bind_device(p->q)) return e;
   int impl = select_impl(p, true);
   if (impl < 0) return impl;
-  if (impl == HSTU_IMPL_UMMA) return attn_umma_bwd(*p, (cudaStream_t)stream);
+  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bwd(*p, (cudaStream_t)stream);
   return attn_generic_bwd(*p, (cudaStream_t)stream);
 }
 

@@ -2,7 +2,7 @@
 //
 // Role: the fully general path of libhstu_b200 -- any dtype (fp32/bf16/fp16), any head dims <= 256 with
 // dqk != dv, every mask option of the reference (targets, max_attn_len, min_full_attn_seq_len, contextual prefix),
-// the delta-q (cached) forward and the research-path relative bias.  The tcgen05/TMA kernels (attn_umma_*.cu)
+// the delta-q (cached) forward and the research-path relative bias.  The wgmma/TMA kernels (attn_wgmma_*.cu)
 // take over for bf16/fp16 at the tensor-core-friendly head dims; this file is what they are validated against
 // on-device at sizes the CPU oracle cannot reach, and what runs fp32 and odd head dims (25, 50, 8 ...).
 //

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libhstu_b200 (sm_100a).
+// Shared device/host helpers for libhstu_b200 (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -12,11 +12,11 @@ void set_error(const char* fmt, ...);
 int attn_generic_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_generic_bwd(const hstu_attn_params& p, cudaStream_t st);
 
-// attn_umma_fwd.cu / attn_umma_bwd.cu
-bool umma_supported(const hstu_attn_params& p, bool bwd);
-size_t umma_workspace_bytes(const hstu_attn_params& p, bool bwd);
-int attn_umma_fwd(const hstu_attn_params& p, cudaStream_t st);
-int attn_umma_bwd(const hstu_attn_params& p, cudaStream_t st);
+// attn_wgmma_fwd.cu / attn_wgmma_bwd.cu
+bool wgmma_supported(const hstu_attn_params& p, bool bwd);
+size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
+int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
+int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
 
 // norm.cu
 int layer_norm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, long long n, int D,

@@ -28,8 +28,8 @@ int norm_mul_dropout_bwd_fast(const void* dout, const void* attn, const void* u,
 constexpr int kNormThreads = 256;
 constexpr int kNormWarps = kNormThreads / 32;
 constexpr int kMaxPerLane = 32;     // 32 lanes * 32 = 1024 elements per normalised vector
-constexpr int kPartialRows = 592;   // backward: 148 SMs * 4 CTAs (each CTA emits one partial row of dw/db)
-constexpr int kFwdGridCap = 2368;   // forward: 148 SMs * 16 CTAs
+constexpr int kPartialRows = 528;   // backward: 132 SMs * 4 CTAs (each CTA emits one partial row of dw/db)
+constexpr int kFwdGridCap = 2112;   // forward: 132 SMs * 16 CTAs
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -828,7 +828,7 @@ static int silu_t(const void* x, const void* dy, void* out, long long n, int col
   const long long total = n * (cols / (v ? VEC : 1));
   const int per_thread = (v && !bwd) ? 4 : 1;  // the kernel's U
   long long blocks = (total + 256 * per_thread - 1) / (256 * per_thread);
-  const long long cap = bwd ? 148 * 16 : 148 * 8;
+  const long long cap = bwd ? 132 * 16 : 132 * 8;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
 #define LAUNCH(VV, BB) silu_kernel<T, VV, BB><<<(int)blocks, 256, 0, st>>>((const T*)x, (const T*)dy, (T*)out, n, cols, xs, dys, os)

@@ -2,10 +2,9 @@
 // 16-bit elements (bf16 / fp16), normalised length 256 (D = H * dv = 256), affine LayerNorm.  Same math and the same dropout
 // function as the general kernels in norm.cu (which remain the path for every other shape); what changes is the instruction count.
 //
-// Why: ncu on the general kernels at the bench shape (profiles/r02_ncu_rowwise.txt) shows them bound by instruction issue, not
-// by HBM: 190 / 270 / 660 / 880 warp instructions per row (LN fwd / LN bwd / output stage fwd / bwd) with the issue slots 60-70 %
-// busy -- per-element bounds predicates, scalar fp32 math, scalar conversions, 64-bit index arithmetic.  Here one lane owns exactly
-// one 16-byte vector of a row (no predicates), the math is packed fp32x2 (FADD2 / FMUL2 / FFMA2), conversions work on pairs, a
+// Why: at the bench shape the general kernels spend their instructions on per-element bounds predicates, scalar conversions and
+// 64-bit index arithmetic rather than on the data they move.  Here one lane owns exactly
+// one 16-byte vector of a row (no predicates), the math works on fp32 pairs, conversions work on pairs, a
 // warp keeps TWO rows in flight and the next rows are prefetched into L2.
 #include "common.cuh"
 
@@ -13,11 +12,18 @@ namespace hstu {
 
 namespace {
 
+// fp32 pair arithmetic, lane by lane with round-to-nearest (sm_90 has no packed fp32x2 instructions)
+__device__ __forceinline__ float2 f2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 f2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 f2_fma(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 constexpr int kFastThreads = 256;
 constexpr int kFastWarps = kFastThreads / 32;
 constexpr int kLen = 256;           // normalised length: 32 lanes x 8 elements
-constexpr int kPartialRowsFast = 592;  // same as norm.cu: 148 SMs x 4 CTAs, one partial row of (dw | db) per CTA
-constexpr int kFwdGridCapFast = 148 * 8;
+constexpr int kPartialRowsFast = 528;  // same as norm.cu: 132 SMs x 4 CTAs, one partial row of (dw | db) per CTA
+constexpr int kFwdGridCapFast = 132 * 8;
 
 template <typename T>
 struct Pair16;
@@ -93,8 +99,8 @@ __device__ __forceinline__ void dropout8(float2 (&v)[4], unsigned long long firs
     const float s1 = (lo >> 16) >= thr ? keep_scale : 0.f;
     const float s2 = (hi & 0xffffu) >= thr ? keep_scale : 0.f;
     const float s3 = (hi >> 16) >= thr ? keep_scale : 0.f;
-    v[2 * g] = __fmul2_rn(v[2 * g], make_float2(s0, s1));
-    v[2 * g + 1] = __fmul2_rn(v[2 * g + 1], make_float2(s2, s3));
+    v[2 * g] = f2_mul(v[2 * g], make_float2(s0, s1));
+    v[2 * g + 1] = f2_mul(v[2 * g + 1], make_float2(s2, s3));
   }
 }
 __device__ __forceinline__ uint32_t drop_threshold(float p) {
@@ -136,7 +142,7 @@ __global__ void __launch_bounds__(kFastThreads) ln_fwd_fast_kernel(const T* __re
 #pragma unroll
     for (int k = 0; k < ROWS; ++k) {
       unpack8<T>(raw[k], v[k]);
-      s[k] = hsum(__fadd2_rn(__fadd2_rn(v[k][0], v[k][1]), __fadd2_rn(v[k][2], v[k][3])));
+      s[k] = hsum(f2_add(f2_add(v[k][0], v[k][1]), f2_add(v[k][2], v[k][3])));
     }
     warp_sum_n<ROWS>(s);
     float mean[ROWS], q[ROWS];
@@ -147,8 +153,8 @@ __global__ void __launch_bounds__(kFastThreads) ln_fwd_fast_kernel(const T* __re
       float2 acc = make_float2(0.f, 0.f);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        v[k][i] = __fadd2_rn(v[k][i], nm);
-        acc = __ffma2_rn(v[k][i], v[k][i], acc);
+        v[k][i] = f2_add(v[k][i], nm);
+        acc = f2_fma(v[k][i], v[k][i], acc);
       }
       q[k] = hsum(acc);
     }
@@ -159,7 +165,7 @@ __global__ void __launch_bounds__(kFastThreads) ln_fwd_fast_kernel(const T* __re
       const float2 r2 = splat(rstd);
       float2 o[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) o[i] = __ffma2_rn(__fmul2_rn(v[k][i], r2), wv[i], bv[i]);
+      for (int i = 0; i < 4; ++i) o[i] = f2_fma(f2_mul(v[k][i], r2), wv[i], bv[i]);
       const long long r = r0 + k * rstep;
       if (ok[k]) {
         st16(y + r * ys + col, pack8<T>(o));
@@ -227,12 +233,12 @@ __global__ void __launch_bounds__(kFastThreads) ln_bwd_fast_kernel(const T* __re
       float2 c1 = make_float2(0.f, 0.f), c2 = make_float2(0.f, 0.f);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        xh[k][i] = __ffma2_rn(xh[k][i], r2, nm);
-        aw[i] = __ffma2_rn(g[i], xh[k][i], aw[i]);
-        ab[i] = __fadd2_rn(ab[i], g[i]);
-        wd[k][i] = __fmul2_rn(g[i], wv[i]);
-        c1 = __ffma2_rn(xh[k][i], wd[k][i], c1);
-        c2 = __fadd2_rn(c2, wd[k][i]);
+        xh[k][i] = f2_fma(xh[k][i], r2, nm);
+        aw[i] = f2_fma(g[i], xh[k][i], aw[i]);
+        ab[i] = f2_add(ab[i], g[i]);
+        wd[k][i] = f2_mul(g[i], wv[i]);
+        c1 = f2_fma(xh[k][i], wd[k][i], c1);
+        c2 = f2_add(c2, wd[k][i]);
       }
       c[2 * k] = hsum(c1);
       c[2 * k + 1] = hsum(c2);
@@ -243,7 +249,7 @@ __global__ void __launch_bounds__(kFastThreads) ln_bwd_fast_kernel(const T* __re
       const float2 c1 = splat(-c[2 * k] * inv_d), c2 = splat(-c[2 * k + 1] * inv_d), r2 = splat(rstd[k]);
       float2 o[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) o[i] = __fmul2_rn(__fadd2_rn(wd[k][i], __ffma2_rn(xh[k][i], c1, c2)), r2);
+      for (int i = 0; i < 4; ++i) o[i] = f2_mul(f2_add(wd[k][i], f2_fma(xh[k][i], c1, c2)), r2);
       if (ok[k]) st16(dx + (r0 + k * rstep) * dxs + col, pack8<T>(o));
     }
   }
@@ -310,7 +316,7 @@ __global__ void __launch_bounds__(kFastThreads) nmd_fwd_fast_kernel(const T* __r
 #pragma unroll
     for (int k = 0; k < ROWS; ++k) {
       unpack8<T>(ar[k], a[k]);
-      s[k] = hsum(__fadd2_rn(__fadd2_rn(a[k][0], a[k][1]), __fadd2_rn(a[k][2], a[k][3])));
+      s[k] = hsum(f2_add(f2_add(a[k][0], a[k][1]), f2_add(a[k][2], a[k][3])));
     }
     warp_sum_n<ROWS>(s);
 #pragma unroll
@@ -320,8 +326,8 @@ __global__ void __launch_bounds__(kFastThreads) nmd_fwd_fast_kernel(const T* __r
       float2 acc = make_float2(0.f, 0.f);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        d[k][i] = __fadd2_rn(a[k][i], nm);
-        acc = __ffma2_rn(d[k][i], d[k][i], acc);
+        d[k][i] = f2_add(a[k][i], nm);
+        acc = f2_fma(d[k][i], d[k][i], acc);
       }
       q[k] = hsum(acc);
     }
@@ -339,8 +345,8 @@ __global__ void __launch_bounds__(kFastThreads) nmd_fwd_fast_kernel(const T* __r
       }
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const float2 nrm = __ffma2_rn(__fmul2_rn(d[k][i], r2), wv[i], bv[i]);
-        y[i] = __fmul2_rn(uu[i], nrm);
+        const float2 nrm = f2_fma(f2_mul(d[k][i], r2), wv[i], bv[i]);
+        y[i] = f2_mul(uu[i], nrm);
         if (CONCAT == 2) a[k][i] = nrm;  // concat_ua: the middle part is LN(attn)
       }
       if (!ok[k]) continue;
@@ -434,8 +440,8 @@ __global__ void __launch_bounds__(kFastThreads, 2) nmd_bwd_fast_kernel(
     float2 c1 = make_float2(0.f, 0.f), c2 = make_float2(0.f, 0.f);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const float2 xhat = __ffma2_rn(a[i], r2, nm);
-      const float2 nrm = __ffma2_rn(xhat, wv[i], bv[i]);
+      const float2 xhat = f2_fma(a[i], r2, nm);
+      const float2 nrm = f2_fma(xhat, wv[i], bv[i]);
       float2 ua = uu[i];
       float2 dsil = make_float2(1.f, 1.f);
       if (silu_u) {
@@ -443,16 +449,16 @@ __global__ void __launch_bounds__(kFastThreads, 2) nmd_bwd_fast_kernel(
         ua = make_float2(uu[i].x * sx, uu[i].y * sy);
         dsil = make_float2(sx * (1.f + uu[i].x * (1.f - sx)), sy * (1.f + uu[i].y * (1.f - sy)));
       }
-      float2 dua = __ffma2_rn(gy[i], nrm, gu[i]);                       // d / d u'
+      float2 dua = f2_fma(gy[i], nrm, gu[i]);                       // d / d u'
       // concat_ua: the gradient of the middle part belongs to LN(attn) and flows through the normalisation
-      const float2 dn = CONCAT == 2 ? __ffma2_rn(gy[i], ua, ga[i]) : __fmul2_rn(gy[i], ua);  // d / d LN(attn)
-      if (silu_u) dua = __fmul2_rn(dua, dsil);
+      const float2 dn = CONCAT == 2 ? f2_fma(gy[i], ua, ga[i]) : f2_mul(gy[i], ua);  // d / d LN(attn)
+      if (silu_u) dua = f2_mul(dua, dsil);
       gu[i] = dua;
-      aw[i] = __ffma2_rn(dn, xhat, aw[i]);
-      ab[i] = __fadd2_rn(ab[i], dn);
-      const float2 wdy = __fmul2_rn(dn, wv[i]);
-      c1 = __ffma2_rn(xhat, wdy, c1);
-      c2 = __fadd2_rn(c2, wdy);
+      aw[i] = f2_fma(dn, xhat, aw[i]);
+      ab[i] = f2_add(ab[i], dn);
+      const float2 wdy = f2_mul(dn, wv[i]);
+      c1 = f2_fma(xhat, wdy, c1);
+      c2 = f2_add(c2, wdy);
       gy[i] = wdy;
       a[i] = xhat;
     }
@@ -462,8 +468,8 @@ __global__ void __launch_bounds__(kFastThreads, 2) nmd_bwd_fast_kernel(
     float2 o[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      o[i] = __fmul2_rn(__fadd2_rn(gy[i], __ffma2_rn(a[i], k1, k2)), r2);
-      if (CONCAT == 1) o[i] = __fadd2_rn(o[i], ga[i]);  // concat_ux: the middle part is attn itself
+      o[i] = f2_mul(f2_add(gy[i], f2_fma(a[i], k1, k2)), r2);
+      if (CONCAT == 1) o[i] = f2_add(o[i], ga[i]);  // concat_ux: the middle part is attn itself
     }
     st16(dattn + r * das + col, pack8<T>(o));
     st16(du + r * dus + col, pack8<T>(gu));

@@ -160,7 +160,7 @@ template <typename T>
 static int position_bwd_t(const void* dout, void* dseq, float* dpos, float* dts, const int* pi, const int* ti, long long L, int D,
                           float alpha, cudaStream_t st) {
   // ~8 CTAs per SM in flight; at least 32 rows per CTA so that the time-bucket runs are worth keeping in registers
-  long long rows = (L + 148 * 8 - 1) / (148 * 8);
+  long long rows = (L + 132 * 8 - 1) / (132 * 8);
   rows = rows < 32 ? 32 : rows;
   const unsigned blocks = (unsigned)((L + rows - 1) / rows);
   const T* d = reinterpret_cast<const T*>(dout);

@@ -3,7 +3,7 @@
 #include <mutex>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hstu {
 
@@ -55,36 +55,6 @@ int make_tmap_rows_heads(CUtensorMap* out, const void* base, long long rows, int
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows=%lld heads=%d d=%d row_stride=%lld head_stride=%lld box=%dx%d)",
               (int)r, rows, heads, d, row_stride, head_stride, box_cols, box_rows);
-    return HSTU_ERR_CUDA;
-  }
-  return 0;
-}
-
-// fp32 [rows, heads, d] contiguous tensor (the dQ accumulator): boxes of box_cols fp32 x box_rows rows of one head, swizzled
-// like the 16-bit operand boxes (box_cols * 4 bytes wide), used as the destination of TMA reduce-add.
-int make_tmap_rows_heads_f32(CUtensorMap* out, const void* base, long long rows, int heads, int d, int box_cols, int box_rows) {
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled is not available from this driver");
-    return HSTU_ERR_CUDA;
-  }
-  const int sw_bytes = box_cols * 4;
-  CUtensorMapSwizzle sw = sw_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                          : sw_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                           : CU_TENSOR_MAP_SWIZZLE_NONE;
-  if (sw == CU_TENSOR_MAP_SWIZZLE_NONE || (reinterpret_cast<uintptr_t>(base) & 15)) {
-    set_error("fp32 tensor map: unsupported box width %d or unaligned base %p", box_cols, base);
-    return HSTU_ERR_UNSUPPORTED;
-  }
-  cuuint64_t dims[3] = {(cuuint64_t)d, (cuuint64_t)heads, (cuuint64_t)rows};
-  cuuint64_t strides[2] = {(cuuint64_t)d * 4, (cuuint64_t)heads * d * 4};
-  cuuint32_t box[3] = {(cuuint32_t)box_cols, 1u, (cuuint32_t)box_rows};
-  cuuint32_t estr[3] = {1u, 1u, 1u};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (fp32) failed with CUresult %d (rows=%lld heads=%d d=%d box=%dx%d)", (int)r, rows, heads, d,
-              box_cols, box_rows);
     return HSTU_ERR_CUDA;
   }
   return 0;

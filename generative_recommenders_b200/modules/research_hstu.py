@@ -1,4 +1,4 @@
-"""Research-path HSTU block on the B200 ops (SURVEY.md section 8 row a11).
+"""Research-path HSTU block on the H100 ops (SURVEY.md section 8 row a11).
 
 Mirrors generative_recommenders/research/modeling/sequential/hstu.py:
   * `RelativeBucketedTimeAndPositionBasedBias` (:87-144) -- here only the parameter container (`_ts_w [num_buckets + 1]`,
@@ -56,7 +56,7 @@ class SequentialTransductionUnitJagged(HammerModule):
         if linear_config != "uvqk":
             raise ValueError(f"Unknown linear_config {linear_config}")
         if normalization not in ("rel_bias", "hstu_rel_bias"):
-            raise NotImplementedError(f"normalization {normalization!r}: only the HSTU (silu) attention is built for B200")
+            raise NotImplementedError(f"normalization {normalization!r}: only the HSTU (silu) attention is built for H100")
         if linear_activation != "silu":
             raise NotImplementedError("linear_activation must be 'silu' (the setting of every reference config)")
         if relative_attention_bias_module is None:

@@ -1,4 +1,4 @@
-"""Sampled-softmax training loss on the B200 ops (SURVEY.md section 8 row f3).
+"""Sampled-softmax training loss on the H100 ops (SURVEY.md section 8 row f3).
 
 Mirrors generative_recommenders/research/modeling/sequential/losses/sampled_softmax.py:29-193 (`SampledSoftmaxLoss`) and the
 sampler it is configured with, autoregressive_losses.py:29-121 (`NegativesSampler`, `LocalNegativesSampler`): same constructor

@@ -1,4 +1,4 @@
-"""HSTU block (STULayer / STUStack) on the B200 ops.
+"""HSTU block (STULayer / STUStack) on the H100 ops.
 
 Parameter names, config fields and forward / cached_forward semantics follow the reference
 generative_recommenders/modules/stu.py:64-466 so that checkpoints (`_uvqk_weight`, `_uvqk_beta`,

@@ -1,4 +1,4 @@
-"""Jagged HSTU attention on B200 -- host side of `hstu_attn_fwd` / `hstu_attn_bwd` (include/hstu_b200.h).
+"""Jagged HSTU attention on H100 -- host side of `hstu_attn_fwd` / `hstu_attn_bwd` (include/hstu_b200.h).
 
 Same call surface as the reference facade generative_recommenders/ops/hstu_attention.py:44-203
 (`hstu_mha`, `delta_hstu_mha`), same argument meaning and assertions; `kernel` must be HammerKernel.CUDA.
@@ -115,10 +115,9 @@ def cuda_hstu_attention_bwd(
     keep = _fill_bias(p, bias, dbias)
     ws = _workspace(p, True, dev)
     with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
-        impl_used = _lib.lib().hstu_attn_select_impl(C.byref(p), 1)
         _lib.check(_lib.lib().hstu_attn_bwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_bwd")
-    # tcgen05 path: max|dO| pre-pass + main kernel + dQ convert; generic path: dK/dV kernel + dQ kernel
-    _lib.note_launch(3 if impl_used == _lib.IMPL_UMMA else 2)
+    # wgmma path: main kernel + dQ convert; generic path: dK/dV kernel + dQ kernel
+    _lib.note_launch(2)
     del ws, keep
 
 

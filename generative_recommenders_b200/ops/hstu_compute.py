@@ -1,4 +1,4 @@
-"""Block-level fused ops of one HSTU layer on B200.
+"""Block-level fused ops of one HSTU layer on H100.
 
 Same surface as generative_recommenders/ops/hstu_compute.py:50-259:
   hstu_compute_uqvk              LN -> addmm -> split [u|v|q|k] -> silu(u)

@@ -1,4 +1,4 @@
-"""Jagged concat / split on B200 -- host side of hstu_jagged_concat / hstu_jagged_split.
+"""Jagged concat / split on H100 -- host side of hstu_jagged_concat / hstu_jagged_split.
 
 Same surface as generative_recommenders/ops/jagged_tensors.py:55-207.  Row routing is integer-exact; the backward of
 concat is split and vice versa (as in ops/triton/triton_jagged_tensors.py:213-244,329-359).

@@ -1,4 +1,4 @@
-"""LayerNorm / SwishLayerNorm / RMSNorm on B200 -- host side of hstu_layer_norm_* / hstu_rms_norm_*.
+"""LayerNorm / SwishLayerNorm / RMSNorm on H100 -- host side of hstu_layer_norm_* / hstu_rms_norm_*.
 
 Same surface as generative_recommenders/ops/layer_norm.py:46-184 (functions + the three HammerModules).
 Statistics and parameter gradients are fp32; outputs keep x.dtype (pt_layer_norm.py:24-61).

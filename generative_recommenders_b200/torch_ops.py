@@ -1,14 +1,14 @@
-"""`torch.ops.hstu.*` registration of the B200 attention: the reference's OWN native operator schema.
+"""`torch.ops.hstu.*` registration of the H100 attention: the reference's OWN native operator schema.
 
 The reference's C++ extension declares three operators in the `hstu` namespace
 (generative_recommenders/ops/cpp/hstu_attention/flash_api.cpp:275-365): `hstu_mha` (autograd), `hstu_mha_fwd`, `hstu_mha_bwd`,
 implemented there for sm80 / sm90.  `register()` defines the same schemas (as a library FRAGMENT, so it coexists with an
 already-loaded reference extension only if that one is absent -- a second definition of the same operator is an error) and
-routes them to libhstu_b200.so, so code written against `torch.ops.hstu.hstu_mha(...)` runs on B200 unchanged.
+routes them to libhstu_b200.so, so code written against `torch.ops.hstu.hstu_mha(...)` runs on H100 unchanged.
 
 Arguments this backend does not implement raise instead of being ignored: `attn_scale`, `q/k/v_descale` (fp8 paths).
 `deterministic=True` selects the CUDA-core backward (query-stationary dQ, no atomics / no reduce-add: bitwise reproducible);
-the default tcgen05 backward accumulates dQ with TMA reduce-adds whose order varies from run to run (fp32, ~1e-7 relative).
+the default wgmma backward accumulates dQ with fp32 atomic adds whose order varies from run to run (fp32, ~1e-7 relative).
 `sort_by_length` / `sm_margin` are accepted and ignored (the kernels always schedule heavy tiles first and use every SM).
 """
 from typing import List, Optional
@@ -34,9 +34,9 @@ _BWD = ("hstu_mha_bwd(int max_seq_len, float alpha, Tensor dout, Tensor q, Tenso
 def _check(causal, seq_offsets, attn_scale, descales):
     torch._assert(causal, "only support causal attention")
     if seq_offsets is None:
-        raise RuntimeError("hstu::hstu_mha on B200: the dense (seq_offsets=None) layout is not implemented; pass jagged tensors")
+        raise RuntimeError("hstu::hstu_mha on H100: the dense (seq_offsets=None) layout is not implemented; pass jagged tensors")
     if attn_scale is not None or any(d is not None for d in descales):
-        raise RuntimeError("hstu::hstu_mha on B200: attn_scale / q,k,v_descale (fp8) are not implemented")
+        raise RuntimeError("hstu::hstu_mha on H100: attn_scale / q,k,v_descale (fp8) are not implemented")
 
 
 def _fwd(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_scale, max_attn_len, min_full_attn_seq_len,

@@ -1,5 +1,5 @@
 /*
- * hstu_b200.h -- C ABI of libhstu_b200.so: the B200 (sm_100a) backend of the HSTU hot path.
+ * hstu_b200.h -- C ABI of libhstu_b200.so: the H100 (sm_90a) backend of the HSTU hot path.
  *
  * Every entry point takes raw device pointers, element strides and sizes -- no ATen / torch types cross
  * this boundary.  All functions return 0 on success and a negative code on failure; the message is
@@ -7,7 +7,7 @@
  * the library never synchronises the device.
  *
  * Reference interfaces each entry point replaces (paths under
- * /root/reference/generative_recommenders/):
+ * generative_recommenders/ of the reference):
  *
  *   hstu_attn_fwd / hstu_attn_bwd
  *        ops/hstu_attention.py:44-128            hstu_mha (python facade, kernel=HammerKernel.CUDA)
@@ -56,9 +56,9 @@ typedef enum hstu_status {
 } hstu_status;
 
 typedef enum hstu_attn_impl {
-  HSTU_IMPL_AUTO = 0,  /* tcgen05/TMA kernels when the shape allows, else the generic kernels */
+  HSTU_IMPL_AUTO = 0,  /* wgmma/TMA kernels when the shape allows, else the generic kernels */
   HSTU_IMPL_GENERIC = 1, /* CUDA-core fp32-accumulate kernels: any dtype / head dim <= 256 / all mask options */
-  HSTU_IMPL_UMMA = 2   /* force tcgen05 + TMA kernels (bf16/fp16, dqk == dv in {32, 64, 128}) */
+  HSTU_IMPL_UMMA = 2   /* force wgmma + TMA kernels (bf16/fp16, dqk == dv in {32, 64, 128, 256}; backward up to 128) */
 } hstu_attn_impl;
 
 /* One jagged attention problem: q,k [L, H, dqk], v [L, H, dv], last-dim stride 1, arbitrary row and head

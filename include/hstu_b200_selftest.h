@@ -1,9 +1,9 @@
 /*
  * hstu_b200_selftest.h -- C ABI of libhstu_b200_selftest.so: TEST INFRASTRUCTURE, not part of the product library.
  *
- * On-device self test and micro-benchmarks of the tcgen05 / TMA primitives the attention kernels of libhstu_b200.so are built
- * from (K-major and MN-major shared-memory descriptors, TMEM load / store, MMA issue rates, commit costs, MUFU and packing
- * rates, the mixed-format probe).  Built from csrc/umma_selftest.cu + csrc/tmap.cu by generative_recommenders_b200/build.py.
+ * On-device self test of the sm_90a primitives the attention kernels of libhstu_b200.so are built from (TMA loads of
+ * swizzled boxes, wgmma with K-major and MN-major shared-memory operands and with A from registers).  Built from
+ * csrc/wgmma_selftest.cu + csrc/tmap.cu by generative_recommenders_b200/build.py.  The entry point keeps its earlier name.
  */
 #ifndef HSTU_B200_SELFTEST_H_
 #define HSTU_B200_SELFTEST_H_
@@ -14,9 +14,7 @@
 extern "C" {
 #endif
 
-/* Writes a report into `report` (host buffer).  Returns the number of failed checks (0 = all good, <0 = could not run).
- * With the environment variable HSTU_SELFTEST_MIXED=1 it runs ONLY the probe of fp16 x bf16 operands in one kind::f16
- * instruction, which raises "illegal instruction" on B200 and poisons the CUDA context: call it from a process of its own. */
+/* Writes a report into `report` (host buffer).  Returns the number of failed checks (0 = all good, <0 = could not run). */
 int hstu_umma_selftest(char* report, size_t report_bytes);
 const char* hstu_selftest_last_error(void);
 

@@ -2,8 +2,8 @@
 jagged ops the reference's PyTorch-eager path calls (plus `jagged_dense_elementwise_add_jagged_output` for ops/position.py).
 
 The reference (generative_recommenders @ 2e81fab) depends on `fbgemm_gpu>=1.1.0`
-(/root/reference/requirements.txt:2), which is a third-party dependency that is NOT
-vendored under /root/reference and is not installable in this container (no network).
+(requirements.txt:2 of the reference), which is a third-party dependency that is NOT
+vendored in the reference repository.
 Its published semantics for the three ops on the hot path are restated here so that the
 *unmodified* reference eager code can be imported and run on CPU to generate the golden
 vectors in tests/golden/ (see tests/golden/make_golden.py).

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY -- CPU restatement of the reference's HSTU hot path.
 
-This file is the *oracle* for the B200 kernels: an independent, per-sequence, fp32/fp64
+This file is the *oracle* for the CUDA kernels: an independent, per-sequence, fp32/fp64
 restatement (torch CPU tensors + numpy integer routing; explicit backward formulas for the
 attention) of the reference's PyTorch-eager path.  It is imported only by `tests/`,
 `__graft_entry__.smoke()` and the `cpu_baseline` / `--impl reference` legs of `bench.py`.
@@ -13,7 +13,7 @@ tests/test_oracle_vs_golden.py.  The third-party fbgemm_gpu jagged ops (>=1.1.0,
 are restated in the shim; that boundary itself is "parity unpinned" by the reference repo.
 
 Every function cites the reference file:line it follows (paths relative to
-/root/reference/generative_recommenders/).
+generative_recommenders/ of the reference).
 """
 from __future__ import annotations
 

@@ -1,17 +1,18 @@
 #!/usr/bin/env python3
-"""Discrete simulation of the mbarrier protocol of attn_bwd_umma_kernel (csrc/attn_umma_bwd.cu) on the CPU.
+"""Discrete simulation of the synchronisation protocol of attn_bwd_wgmma_kernel (csrc/attn_wgmma_bwd.cu) on the CPU.
 
-Checks, under random schedules, that (1) nobody deadlocks, (2) no parity wait "passes falsely" -- a waiter asking for
-phase k of a barrier while phase k-1 has not completed sees the parity test succeed at once -- and (3) no waiter falls two
-phases behind (its parity test would then block until the barrier wraps).  Both bugs happened on the GPU during
-development (unit_done with a 3-slot ring; s_full with a single slot); this model reproduces them when the fix is removed
-(--break-ud / --break-sf).
+Checks, under random schedules, that (1) nobody deadlocks, (2) no mbarrier parity wait "passes falsely" -- a waiter asking
+for phase k while phase k-1 has not completed sees the parity test succeed at once --, (3) no waiter falls two phases behind,
+(4) no TMA load is issued into a Q / dO stage that a warpgroup still reads, and (5) no dS buffer is written while the dQ
+MMA of an earlier tile reads it, or read while it is written.
 
-Actors: X (scores), YV (dV), YK (dK), Z (dQ) issuers, two elementwise warpgroups W0 / W1, D the dQ drain warpgroup whose elected
-lane is also the TMA producer.  tcgen05.commit and TMA completions are asynchronous: they are queued per issuing actor and
-fire later, in order.
-usage: sim_bwd_protocol.py [--d 32|64|128] [--tiles T] [--seeds N] [--break-ud] [--break-sf]"""
-import argparse, random
+Actors: the two warpgroups W0 / W1 (128 threads each, modelled as one arrival each); thread 0 of W0 also issues the TMA loads.
+TMA completions are asynchronous: queued per issuing actor and fired later, in order.
+usage: sim_bwd_protocol.py [--d 32|64|128] [--tiles T] [--seeds N] [--break-ds]"""
+import argparse
+import random
+
+STAGES = {32: 4, 64: 3, 128: 2}  # BwdCfg<D>::STAGES
 
 
 class Bar:
@@ -28,191 +29,10 @@ class Violation(Exception):
     pass
 
 
-def cfg_for(d):
-    # the product configuration: Q / dO stages, score slots (P^T written over the scores of its unit), dQ accumulators
-    return dict(NST={32: 4, 64: 3, 128: 1}[d], NSLOT={32: 3, 64: 2, 128: 1}[d], NDQ={32: 2, 64: 2, 128: 1}[d])
-
-
-def run_pring(T, d, seed):
-    """PRING mode of the kernel (d <= 64): one score slot per warpgroup, handed back right after the load; P^T ring of NPR
-    buffers released by the dV commits; NDQ dQ accumulators."""
-    NST = {32: 4, 64: 3}[d]
-    NPR = {32: 4, 64: 2}[d]
-    NDQ = {32: 2, 64: 1}[d]
-    rnd = random.Random(seed)
-    B = {"kv": Bar(1), "kvr": Bar(1), "fin": Bar(2)}
-    for i in range(4):
-        B[f"qf{i}"], B[f"qr{i}"], B[f"td{i}"], B[f"ud{i}"], B[f"pf{i}"] = Bar(1), Bar(1), Bar(3), Bar(1), Bar(1)
-    for i in range(2):
-        B[f"sf{i}"], B[f"free{i}"], B[f"dqe{i}"] = Bar(1), Bar(1), Bar(1)
-    U = 2 * T
-
-    def ud(u):
-        i, hf = u >> 1, u & 1
-        return f"ud{hf * 2 + (i & 1)}", i >> 1
-
-    def X():
-        yield ("wait", "kvr", 0)
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            if i >= 1:
-                yield ("wait", f"free{hf}", i - 1)
-            if hf == 0:
-                yield ("wait", f"qr{i % NST}", i // NST)
-            yield ("async", f"sf{hf}")
-
-    def YV():
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            yield ("wait",) + ud(u)
-            yield ("async", f"pf{u % NPR}")
-            if hf == 1:
-                yield ("async", f"td{i & 3}")
-        yield ("async", "fin")
-
-    def YK():
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            yield ("wait",) + ud(u)
-            if hf == 1:
-                yield ("async", f"td{i & 3}")
-        yield ("async", "fin")
-
-    def Z():
-        yield ("wait", "kvr", 0)
-        for i in range(T):
-            yield ("wait",) + ud(2 * i)
-            yield ("wait",) + ud(2 * i + 1)
-            if i >= NDQ:
-                yield ("wait", f"dqe{i % NDQ}", i // NDQ - 1)
-            yield ("async", f"td{i & 3}")
-
-    def W(h):
-        for i in range(T):
-            u = 2 * i + h
-            yield ("wait", f"sf{h}", i)
-            yield ("arrive", f"free{h}")     # all scores loaded: the slot goes back to the issuer
-            if i >= 2:
-                yield ("wait", f"td{(i - 2) & 3}", (i - 2) >> 2)
-            if u >= NPR:
-                yield ("wait", f"pf{u % NPR}", u // NPR - 1)
-            yield ("arrive", ud(u)[0])
-        yield ("wait", "fin", 0)
-
-    def Dr():
-        yield ("async", "kv")
-        for i in range(min(NST, T)):
-            yield ("async", f"qf{i % NST}")
-        yield ("wait", "kv", 0)
-        yield ("arrive", "kvr")
-        for i in range(min(NST, T)):
-            yield ("wait", f"qf{i % NST}", i // NST)
-            yield ("arrive", f"qr{i % NST}")
-        for i in range(T):
-            yield ("wait", f"td{i & 3}", i >> 2)
-            if i + NST < T:
-                yield ("async", f"qf{(i + NST) % NST}")
-            yield ("arrive", f"dqe{i % NDQ}")
-            t = i - 1 + NST          # the tile whose load was issued one iteration ago
-            if i >= 1 and t < T:
-                yield ("wait", f"qf{t % NST}", t // NST)
-                yield ("arrive", f"qr{t % NST}")
-
-    actors = {"X": X(), "YV": YV(), "YK": YK(), "Z": Z(), "W0": W(0), "W1": W(1), "D": Dr()}
-    return _simulate(actors, B, rnd)
-
-
-def run_psm(T, seed, NST=4, NPB=3, NDQ=2):
-    """PSM mode (d = 32, -DHSTU_BWD_PSMEM): three elementwise warpgroups (unit u -> warpgroup u % 3 -> score slot u % 3), the slot is
-    handed back right after the load (scores_free), P^T goes to a ring of NPB shared-memory boxes released by the dV commits."""
-    rnd = random.Random(seed)
-    B = {"kv": Bar(1), "kvr": Bar(1), "fin": Bar(2)}
-    for i in range(4):
-        B[f"qf{i}"], B[f"qr{i}"], B[f"td{i}"], B[f"ud{i}"], B[f"pf{i}"] = Bar(1), Bar(1), Bar(3), Bar(1), Bar(1)
-    for i in range(3):
-        B[f"sf{i}"], B[f"free{i}"] = Bar(1), Bar(1)
-    for i in range(2):
-        B[f"dqe{i}"] = Bar(1)
-    U = 2 * T
-
-    def ud(u):
-        i, hf = u >> 1, u & 1
-        return f"ud{hf * 2 + (i & 1)}", i >> 1
-
-    def X():
-        yield ("wait", "kvr", 0)
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            if u >= 3:
-                yield ("wait", f"free{u % 3}", u // 3 - 1)
-            if hf == 0:
-                yield ("wait", f"qr{i % NST}", i // NST)
-            yield ("async", f"sf{u % 3}")
-
-    def YV():
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            yield ("wait",) + ud(u)
-            yield ("async", f"pf{u % NPB}")
-            if hf == 1:
-                yield ("async", f"td{i & 3}")
-        yield ("async", "fin")
-
-    def YK():
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            yield ("wait",) + ud(u)
-            if hf == 1:
-                yield ("async", f"td{i & 3}")
-        yield ("async", "fin")
-
-    def Z():
-        yield ("wait", "kvr", 0)
-        for i in range(T):
-            yield ("wait",) + ud(2 * i)
-            yield ("wait",) + ud(2 * i + 1)
-            if i >= NDQ:
-                yield ("wait", f"dqe{i % NDQ}", i // NDQ - 1)
-            yield ("async", f"td{i & 3}")
-
-    def W(w):
-        for u in range(w, U, 3):
-            i = u >> 1
-            yield ("wait", f"sf{w}", u // 3)
-            if i >= 2:
-                yield ("wait", f"td{(i - 2) & 3}", (i - 2) >> 2)
-            if u >= NPB:
-                yield ("wait", f"pf{u % NPB}", u // NPB - 1)
-            yield ("arrive", f"free{w}")     # second chunk loaded: the slot goes back to the issuer
-            yield ("arrive", ud(u)[0])
-        yield ("wait", "fin", 0)
-
-    def Dr():
-        yield ("async", "kv")
-        for i in range(min(NST, T)):
-            yield ("async", f"qf{i % NST}")
-        yield ("wait", "kv", 0)
-        yield ("arrive", "kvr")
-        for i in range(min(NST, T)):
-            yield ("wait", f"qf{i % NST}", i // NST)
-            yield ("arrive", f"qr{i % NST}")
-        for i in range(T):
-            yield ("wait", f"td{i & 3}", i >> 2)
-            if i + NST < T:
-                yield ("async", f"qf{(i + NST) % NST}")
-            yield ("arrive", f"dqe{i % NDQ}")
-            t = i - 1 + NST
-            if i >= 1 and t < T:
-                yield ("wait", f"qf{t % NST}", t // NST)
-                yield ("arrive", f"qr{t % NST}")
-
-    actors = {"X": X(), "YV": YV(), "YK": YK(), "Z": Z(), "W0": W(0), "W1": W(1), "W2": W(2), "D": Dr()}
-    return _simulate(actors, B, rnd)
-
-
 def _simulate(actors, B, rnd):
     pending = {k: None for k in actors}
     queues = {k: [] for k in actors}
+    readers, writers = {}, {}   # resource -> number of actors inside a read / write of it
     done = set()
     steps = 0
     while len(done) < len(actors) or any(queues.values()):
@@ -249,149 +69,20 @@ def _simulate(actors, B, rnd):
                 B[op[1]].arrive()
             elif op[0] == "async":
                 queues[k].append(op[1])
-            pending[k] = None
-            progressed = True
-            break
-        if not progressed:
-            state = {k: pending[k] for k in actors if k not in done}
-            raise Violation(f"deadlock: {state}")
-    return steps
-
-
-def run(T, d, seed, break_ud=False, break_sf=False):
-    c = cfg_for(d)
-    NST, NSLOT, NDQ = c["NST"], c["NSLOT"], c["NDQ"]
-    NSF = NSLOT if break_sf else max(NSLOT, 2)
-    LAG = NDQ
-    rnd = random.Random(seed)
-    B = {"kv": Bar(1), "kvr": Bar(1), "fin": Bar(2)}
-    for i in range(4):
-        B[f"qf{i}"] = Bar(1)
-        B[f"qr{i}"] = Bar(2 if NST == 1 else 1)  # bf16 inputs: tile converted to fp16 (by the drain warpgroup, or -- single
-        #                                             stage -- by the two elementwise warpgroups: one arrival each)
-        B[f"td{i}"] = Bar(3)       # YV, YK, Z
-        B[f"ud{i}"] = Bar(1)       # count 128 threads modelled as one arrival per warpgroup
-    for i in range(3):
-        B[f"sf{i}"] = Bar(1)
-        B[f"free{i}"] = Bar(1)
-    for i in range(2):
-        B[f"dqe{i}"] = Bar(1)      # the drain warpgroup (128 threads modelled as one arrival)
-    U = 2 * T
-
-    def ud(u):  # barrier instance and phase index of unit_done for unit u
-        i, hf = u >> 1, u & 1
-        if break_ud:
-            return f"ud{hf}", i                     # one barrier per half: aliases with a 3-slot ring
-        return f"ud{hf * 2 + (i & 1)}", i >> 1
-
-    def X():
-        yield ("wait", "kvr", 0)
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            if u >= NSLOT:
-                yield ("wait", f"free{u % NSLOT}", u // NSLOT - 1)
-            if hf == 0:
-                yield ("wait", f"qr{i % NST}", i // NST)
-            yield ("async", f"sf{u % NSF}")
-
-    def YV():
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            yield ("wait",) + ud(u)
-            yield ("async", f"free{u % NSLOT}")
-            if hf == 1:
-                yield ("async", f"td{i & 3}")
-        yield ("async", "fin")
-
-    def YK():
-        for u in range(U):
-            i, hf = u >> 1, u & 1
-            yield ("wait",) + ud(u)
-            if hf == 1:
-                yield ("async", f"td{i & 3}")
-        yield ("async", "fin")
-
-    def Z():
-        yield ("wait", "kvr", 0)
-        for i in range(T):
-            yield ("wait",) + ud(2 * i)
-            yield ("wait",) + ud(2 * i + 1)
-            if i >= NDQ:
-                yield ("wait", f"dqe{i % NDQ}", i // NDQ - 1)
-            yield ("async", f"td{i & 3}")
-
-    def W(h):
-        for i in range(T):
-            u = 2 * i + h
-            if NST == 1:             # single stage: the elementwise warpgroups convert the tile that has just landed
-                yield ("wait", "qf0", i)
-                yield ("arrive", "qr0")
-            yield ("wait", f"sf{u % NSF}", u // NSF)
-            if i >= 2:
-                yield ("wait", f"td{(i - 2) & 3}", (i - 2) >> 2)
-            yield ("arrive", ud(u)[0])
-        yield ("wait", "fin", 0)
-
-    def Dr():  # the bf16 variant (with the in-place conversion); fp16 inputs are the same protocol without the qr hops
-        yield ("async", "kv")
-        for i in range(min(NST, T)):
-            yield ("async", f"qf{i % NST}")
-        yield ("wait", "kv", 0)
-        yield ("arrive", "kvr")
-        if NST > 1:
-            for i in range(min(NST, T)):
-                yield ("wait", f"qf{i % NST}", i // NST)
-                yield ("arrive", f"qr{i % NST}")
-        for i in range(T):
-            yield ("wait", f"td{i & 3}", i >> 2)
-            if i + NST < T:
-                yield ("async", f"qf{(i + NST) % NST}")
-            yield ("arrive", f"dqe{i % NDQ}")
-            # four stages: convert the tile whose load was issued one iteration ago; three: the one just issued (blocking)
-            t = i - 1 + NST if NST >= 4 else i + NST
-            if NST > 1 and (i >= 1 or NST < 4) and t < T:
-                yield ("wait", f"qf{t % NST}", t // NST)
-                yield ("arrive", f"qr{t % NST}")
-
-    actors = {"X": X(), "YV": YV(), "YK": YK(), "Z": Z(), "W0": W(0), "W1": W(1), "D": Dr()}
-    pending = {k: None for k in actors}     # the blocking wait of each actor
-    queues = {k: [] for k in actors}        # asynchronous completions (commit / TMA), in order per actor
-    done = set()
-    steps = 0
-    while len(done) < len(actors) or any(queues.values()):
-        steps += 1
-        if steps > 200000:
-            raise Violation("no progress (livelock?)")
-        choices = [("run", k) for k in actors if k not in done] + [("fire", k) for k, q in queues.items() if q]
-        rnd.shuffle(choices)
-        progressed = False
-        for kind, k in choices:
-            if kind == "fire":
-                B[queues[k].pop(0)].arrive()
-                progressed = True
-                break
-            if pending[k] is None:
-                try:
-                    pending[k] = next(actors[k])
-                except StopIteration:
-                    done.add(k)
-                    progressed = True
-                    break
-            op = pending[k]
-            if op[0] == "wait":
-                _, name, want = op
-                bar = B[name]
-                passes = (bar.phase & 1) != (want & 1)          # try_wait.parity semantics
-                if passes and bar.phase <= want:
-                    raise Violation(f"{k}: wait on {name} for phase {want} passed while the barrier is in phase {bar.phase} (false pass)")
-                if not passes and bar.phase > want:
-                    raise Violation(f"{k}: wait on {name} for phase {want} but the barrier is already in phase {bar.phase} (two ahead)")
-                if not passes:
-                    continue
-            elif op[0] == "arrive":
-                B[op[1]].arrive()
-            elif op[0] == "async":
+            elif op[0] == "tma":          # TMA load into stage op[2], completing on barrier op[1]
+                if readers.get(op[2], 0):
+                    raise Violation(f"{k}: TMA load into {op[2]} while it is being read")
                 queues[k].append(op[1])
+            elif op[0] in ("read", "write"):
+                _, res, delta = op
+                if op[0] == "read":
+                    if writers.get(res, 0):
+                        raise Violation(f"{k}: reads {res} while it is being written")
+                    readers[res] = readers.get(res, 0) + delta
+                else:
+                    if readers.get(res, 0):
+                        raise Violation(f"{k}: writes {res} while it is being read")
+                    writers[res] = writers.get(res, 0) + delta
             pending[k] = None
             progressed = True
             break
@@ -401,28 +92,54 @@ def run(T, d, seed, break_ud=False, break_sf=False):
     return steps
 
 
-def run_variant_pring(T, d, seed):
-    """The PRING variant (compile with -DHSTU_BWD_PRING=1): measured slower than the default on B200, kept switchable."""
-    return run_pring(T, d, seed)
+def run(T, d, seed, break_ds=False):
+    """One key-tile CTA streaming T query tiles.  break_ds: one dS buffer instead of two (must be caught)."""
+    NST = STAGES[d]
+    NDS = 1 if break_ds else 2
+    rnd = random.Random(seed)
+    B = {"kv": Bar(1), "nb": Bar(2)}
+    for i in range(NST):
+        B[f"qf{i}"] = Bar(1)   # expect_tx arrival of thread 0 + TMA bytes: modelled as the TMA completion
+        B[f"qe{i}"] = Bar(2)   # 256 consumer threads: one arrival per warpgroup
+
+    def W(w):
+        if w == 0:                                   # thread 0: K / V and the first STAGES query tiles
+            yield ("async", "kv")
+            for j in range(min(T, NST)):
+                yield ("tma", f"qf{j % NST}", f"q{j % NST}")
+        yield ("wait", "kv", 0)
+        for j in range(T):
+            st = j % NST
+            yield ("wait", f"qf{st}", j // NST)
+            yield ("read", f"q{st}", 1)              # S^T, dP^T, dV, dK MMAs read Q_j / dO_j ...
+            yield ("read", f"q{st}", -1)             # ... and complete within the iteration
+            yield ("arrive", f"qe{st}")
+            if w == 0 and j + NST < T:               # refill the stage once both warpgroups have released it
+                yield ("wait", f"qe{st}", j // NST)
+                yield ("tma", f"qf{st}", f"q{st}")
+            b = f"ds{j % NDS}"
+            yield ("write", b, 1)                    # dS^T of this warpgroup's 64 keys
+            yield ("write", b, -1)
+            yield ("arrive", "nb")                   # named barrier of the 256 consumer threads
+            yield ("wait", "nb", j)
+            if j % 2 == w:                           # dQ_j = dS K, waited for before the warpgroup goes on
+                yield ("read", b, 1)
+                yield ("read", b, -1)
+
+    return _simulate({"W0": W(0), "W1": W(1)}, B, rnd)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--d", type=int, default=32, choices=sorted(STAGES))
+    ap.add_argument("--tiles", type=int, default=8)
+    ap.add_argument("--seeds", type=int, default=200)
+    ap.add_argument("--break-ds", action="store_true")
+    a = ap.parse_args()
+    for s in range(a.seeds):
+        run(a.tiles, a.d, s, break_ds=a.break_ds)
+    print(f"ok: d={a.d} tiles={a.tiles} seeds={a.seeds}")
 
 
 if __name__ == "__main__":
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--d", type=int, default=0)
-    ap.add_argument("--tiles", type=int, default=0)
-    ap.add_argument("--seeds", type=int, default=200)
-    ap.add_argument("--break-ud", action="store_true")
-    ap.add_argument("--break-sf", action="store_true")
-    a = ap.parse_args()
-    bad = 0
-    for d in ([a.d] if a.d else [32, 64, 128]):
-        for T in ([a.tiles] if a.tiles else [1, 2, 3, 4, 5, 8, 13, 64]):
-            for seed in range(a.seeds):
-                try:
-                    run(T, d, seed, a.break_ud, a.break_sf)
-                except Violation as e:
-                    bad += 1
-                    if bad <= 5:
-                        print(f"d={d} T={T} seed={seed}: {e}")
-    print("violations:", bad)
-    raise SystemExit(1 if bad else 0)
+    main()

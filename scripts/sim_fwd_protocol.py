@@ -1,130 +1,76 @@
 #!/usr/bin/env python3
-"""Discrete simulation of the mbarrier protocol of the PERSISTENT forward kernel (attn_fwd_umma_persist_kernel, csrc/attn_umma_fwd.cu).
+"""Discrete simulation of the synchronisation protocol of attn_fwd_wgmma_kernel (csrc/attn_wgmma_fwd.cu) on the CPU, on the
+engine of sim_bwd_protocol.py: no deadlock, no mbarrier parity aliasing, and no TMA load into a K or V stage that a warpgroup
+still reads.
 
-One CTA walks a list of work items; item k has T_k key tiles (0 = skipped by every role).  All ring stages, score slots and barrier
-phases run on a global key-tile counter g; Q buffers / O accumulator sets on the count n of non-empty items.  The model checks, under
-random schedules, what scripts/sim_bwd_protocol.py checks for the backward: no deadlock, no parity wait that passes falsely, no waiter
-two phases behind.  Actors: KP (TMA: Q + K tiles), VP (TMA: V tiles), CV (bf16 -> fp16 converter), QK and PV (MMA issuers; commits are
-asynchronous), W0 / W1 (silu warpgroups: key tiles with g % 2 == w, then half of the epilogue each).
-usage: sim_fwd_protocol.py [--seeds N]"""
+Actors: the two warpgroups W0 / W1 (one arrival each on the 256-count empty barriers); thread 0 of W0 issues the TMA loads of
+Q, of the first STAGES key tiles and, once both warpgroups have released stage i % STAGES, of key tile i + STAGES.
+usage: sim_fwd_protocol.py [--d 32|64|128|256] [--tiles T] [--seeds N] [--break-refill]"""
 import argparse
 import importlib.util
 import os
 import random
 
-_spec = importlib.util.spec_from_file_location("sim_bwd_protocol", os.path.join(os.path.dirname(os.path.abspath(__file__)), "sim_bwd_protocol.py"))
-_b = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(_b)
-Bar, Violation, _simulate = _b.Bar, _b.Violation, _b._simulate
+_spec = importlib.util.spec_from_file_location("sim_bwd_protocol", os.path.join(os.path.dirname(os.path.abspath(__file__)),
+                                                                                 "sim_bwd_protocol.py"))
+_eng = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(_eng)
+Bar, Violation = _eng.Bar, _eng.Violation
+
+STAGES = {32: 3, 64: 3, 128: 3, 256: 2}  # FwdCfg<D>::STAGES
 
 
-def run(items, seed, conv=True, NQ=2, NO=2):
-    """items: list of key-tile counts per work item; NQ Q buffers and NO O accumulator sets (2 / 2 for d <= 64, 1 / 1 for d = 128)."""
+def run(T, d, seed, break_refill=False):
+    """One query-tile CTA over T key tiles.  break_refill: thread 0 refills a stage without waiting for its release."""
+    NST = STAGES[d]
     rnd = random.Random(seed)
-    B = {}
-    for i in range(2):
-        B[f"qf{i}"], B[f"qe{i}"], B[f"of{i}"] = Bar(1), Bar(1), Bar(1)
-        B[f"oe{i}"] = Bar(2)             # 256 threads modelled as one arrival per warpgroup
-    for i in range(3):
-        B[f"kf{i}"], B[f"vf{i}"], B[f"vr{i}"], B[f"sf{i}"], B[f"pf{i}"], B[f"pd{i}"] = Bar(1), Bar(1), Bar(1), Bar(1), Bar(1), Bar(1)
-    vrdy = "vr" if conv else "vf"
+    B = {"q": Bar(1)}
+    for i in range(NST):
+        B[f"kf{i}"], B[f"vf{i}"] = Bar(1), Bar(1)
+        B[f"ke{i}"], B[f"ve{i}"] = Bar(2), Bar(2)
 
-    def walk():
-        g0 = n = 0
-        for T in items:
-            if T == 0:
-                continue
-            yield g0, n, T
-            g0 += T
-            n += 1
-
-    def KP():
-        for g0, n, T in walk():
-            qb = n % NQ
-            if n >= NQ:
-                yield ("wait", f"qe{qb}", n // NQ - 1)
-            yield ("async", f"qf{qb}")
-            for i in range(T):
-                g = g0 + i
-                if g >= 3:
-                    yield ("wait", f"sf{g % 3}", g // 3 - 1)
-                yield ("async", f"kf{g % 3}")
-
-    def VP():
-        for g0, n, T in walk():
-            for i in range(T):
-                g = g0 + i
-                if g >= 3:
-                    yield ("wait", f"pd{g % 3}", g // 3 - 1)
-                yield ("async", f"vf{g % 3}")
-
-    def CV():
-        for g0, n, T in walk():
-            for i in range(T):
-                g = g0 + i
-                yield ("wait", f"vf{g % 3}", g // 3)
-                yield ("arrive", f"vr{g % 3}")
-
-    def QK():
-        for g0, n, T in walk():
-            yield ("wait", f"qf{n % NQ}", n // NQ)
-            for i in range(T):
-                g = g0 + i
-                if g >= 3:
-                    yield ("wait", f"pd{g % 3}", g // 3 - 1)
-                yield ("wait", f"kf{g % 3}", g // 3)
-                yield ("async", f"sf{g % 3}")
-                if i == T - 1:
-                    yield ("async", f"qe{n % NQ}")
-
-    def PV():
-        for g0, n, T in walk():
-            if n >= NO:
-                yield ("wait", f"oe{n % NO}", n // NO - 1)
-            for i in range(T):
-                g = g0 + i
-                yield ("wait", f"pf{g % 3}", g // 3)
-                yield ("wait", f"{vrdy}{g % 3}", g // 3)
-                yield ("async", f"pd{g % 3}")
-                if i == T - 1:
-                    yield ("async", f"of{n % NO}")
+    def load(i):
+        st = i % NST
+        if i >= NST and not break_refill:
+            yield ("wait", f"ke{st}", i // NST - 1)
+        yield ("tma", f"kf{st}", f"k{st}")
+        if i >= NST and not break_refill:
+            yield ("wait", f"ve{st}", i // NST - 1)
+        yield ("tma", f"vf{st}", f"v{st}")
 
     def W(w):
-        for g0, n, T in walk():
-            for i in range(T):
-                g = g0 + i
-                if (g & 1) != w:
-                    continue
-                yield ("wait", f"sf{g % 3}", g // 3)
-                yield ("arrive", f"pf{g % 3}")
-            yield ("wait", f"of{n % NO}", n // NO)
-            yield ("arrive", f"oe{n % NO}")
+        if w == 0:
+            yield ("async", "q")
+            for i in range(min(T, NST)):
+                yield from load(i)
+        yield ("wait", "q", 0)
+        for i in range(T):
+            st = i % NST
+            yield ("wait", f"kf{st}", i // NST)
+            yield ("read", f"k{st}", 1)          # S = Q K^T, waited for
+            yield ("read", f"k{st}", -1)
+            yield ("arrive", f"ke{st}")
+            yield ("wait", f"vf{st}", i // NST)
+            yield ("read", f"v{st}", 1)          # O += P V, waited for
+            yield ("read", f"v{st}", -1)
+            yield ("arrive", f"ve{st}")
+            if w == 0 and i + NST < T:
+                yield from load(i + NST)
 
-    actors = {"KP": KP(), "VP": VP(), "QK": QK(), "PV": PV(), "W0": W(0), "W1": W(1)}
-    if conv:
-        actors["CV"] = CV()
-    return _simulate(actors, B, rnd)
+    return _eng._simulate({"W0": W(0), "W1": W(1)}, B, rnd)
 
 
-def item_lists(rnd, count):
-    for _ in range(count):
-        n = rnd.randint(1, 12)
-        yield [rnd.choice([0, 1, 1, 2, 3, 4, 7]) for _ in range(n)]
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--d", type=int, default=32, choices=sorted(STAGES))
+    ap.add_argument("--tiles", type=int, default=8)
+    ap.add_argument("--seeds", type=int, default=200)
+    ap.add_argument("--break-refill", action="store_true")
+    a = ap.parse_args()
+    for s in range(a.seeds):
+        run(a.tiles, a.d, s, break_refill=a.break_refill)
+    print(f"ok: d={a.d} tiles={a.tiles} seeds={a.seeds}")
 
 
 if __name__ == "__main__":
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--seeds", type=int, default=300)
-    a = ap.parse_args()
-    rnd = random.Random(1)
-    bad = 0
-    for items in list(item_lists(rnd, 40)) + [[1] * 9, [4] * 5, [64, 1, 64], [0, 0, 3]]:
-        for seed in range(a.seeds // 20):
-            for conv, nq in ((True, 2), (False, 2), (True, 1)):
-                try:
-                    run(items, seed, conv, nq, nq)
-                except Violation as e:
-                    bad += 1
-                    print(items, seed, conv, e)
-    print("violations:", bad)
-    raise SystemExit(1 if bad else 0)
+    main()

@@ -1,13 +1,13 @@
-"""Generate golden vectors from the UNMODIFIED reference eager path (run in the build container).
+"""Generate golden vectors from the UNMODIFIED reference eager path.
 
-    python tests/golden/make_golden.py          # needs /root/reference; writes tests/golden/*.pt
+    python tests/golden/make_golden.py   # checkout at /root/reference, or HSTU_REFERENCE_ROOT=<checkout>; writes tests/golden/*.pt
 
 The reference ships no golden vectors for the HSTU hot path (SURVEY.md section 8c); these fixtures are
 outputs of the reference's own PyTorch-eager code (generative_recommenders @ 2e81fab, imported from
-/root/reference) on seeded inputs, with the three fbgemm_gpu jagged ops supplied by
+a checkout of it) on seeded inputs, with the three fbgemm_gpu jagged ops supplied by
 oracle/fbgemm_shim.py.  They pin the CPU oracle (tests/test_oracle_vs_golden.py) and, through it and
-directly, the CUDA kernels (tests/test_gpu_*.py).  /root/reference does not exist on the GPU box; only
-these committed fixtures travel.
+directly, the CUDA kernels (tests/test_gpu_*.py).  The tests need no checkout of the reference: only
+these committed fixtures.
 """
 import os
 import random
@@ -16,7 +16,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+REF_ROOT = os.environ.get("HSTU_REFERENCE_ROOT") or "/root/reference"
+if not os.path.isdir(os.path.join(REF_ROOT, "generative_recommenders")):
+    sys.exit(f"make_golden.py: no checkout of generative-recommenders at {REF_ROOT} (set HSTU_REFERENCE_ROOT)")
+sys.path.insert(0, REF_ROOT)
 
 from oracle import fbgemm_shim  # noqa: E402
 

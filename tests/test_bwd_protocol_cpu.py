@@ -1,5 +1,6 @@
-"""The mbarrier protocol of the tcgen05 backward kernel, model-checked on the CPU under random schedules
-(scripts/sim_bwd_protocol.py mirrors the waits / arrives / commits of csrc/attn_umma_bwd.cu for d = 32, 64, 128)."""
+"""The synchronisation protocol of the wgmma backward kernel, model-checked on the CPU under random schedules
+(scripts/sim_bwd_protocol.py mirrors the mbarrier waits / arrives, TMA loads, named barrier and dS buffers of
+csrc/attn_wgmma_bwd.cu for d = 32, 64, 128)."""
 import importlib.util
 import os
 
@@ -18,26 +19,9 @@ def test_protocol_has_no_deadlock_or_phase_aliasing(d):
             sim.run(tiles, d, seed)
 
 
-@pytest.mark.parametrize("d", [32, 64])
-def test_pring_variant_protocol(d):
-    for tiles in (1, 2, 3, 5, 8, 21):
-        for seed in range(15):
-            sim.run_variant_pring(tiles, d, seed)
-
-
-def test_psm_mode_protocol():
-    """d = 32 with three elementwise warpgroups and the P^T boxes in shared memory (-DHSTU_BWD_PSMEM)."""
-    for tiles in (1, 2, 3, 4, 5, 7, 8, 13, 64):
-        for seed in range(25):
-            sim.run_psm(tiles, seed)
-
-
-def test_model_reproduces_the_two_bugs_found_on_the_gpu():
-    # one s_full barrier with a single score slot: warpgroup 1 asks for phase 1 before phase 0 completed
-    with pytest.raises(sim.Violation, match="false pass"):
-        for seed in range(40):
-            sim.run(2, 128, seed, break_sf=True)
-    # one unit_done barrier per half with a 3-slot ring: an issuer falls two phases behind
-    with pytest.raises(sim.Violation):
-        for seed in range(200):
-            sim.run(4, 32, seed, break_ud=True)
+@pytest.mark.parametrize("d", [32, 64, 128])
+def test_model_catches_a_single_ds_buffer(d):
+    """With one dS buffer instead of two, a warpgroup overwrites dS while the other one's dQ MMA still reads it."""
+    with pytest.raises(sim.Violation, match="ds0"):
+        for seed in range(100):
+            sim.run(8, d, seed, break_ds=True)

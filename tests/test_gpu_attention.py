@@ -121,7 +121,7 @@ def test_attention_random_grid_generic(idx):
 @pytest.mark.parametrize("opts", [(False, False, 0, 0), (True, False, 0, 0), (True, True, 0, 0), (True, True, 7, 0),
                                   (True, True, 5, 33), (False, False, 4, 0)])
 def test_attention_umma_vs_oracle(d, dtype, opts):
-    """tcgen05/TMA forward (+ backward of whichever implementation AUTO selects) against the fp32 oracle."""
+    """wgmma/TMA forward (+ backward of whichever implementation AUTO selects) against the fp32 oracle."""
     _lib = _mods()[0]
     targets, window, ctx, min_full = opts
     case = _random_case(7000 + d + ctx, dtype, 5, 3, 300, 24, d, d, targets, window, ctx, min_full)

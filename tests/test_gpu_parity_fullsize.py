@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05/TMA attention kernels against the CPU oracle AT THE SHAPES THAT ARE BENCHMARKED
+"""GPU parity of the wgmma/TMA attention kernels against the CPU oracle AT THE SHAPES THAT ARE BENCHMARKED
 (BASELINE.json: d = 32 at Lmax = 8192 is the HSTU-large headline; d = 64 / 128 / 256 are the microbench grid), and of the
 bf16 STU stack (forward, dx and every parameter gradient) in the configuration bench.py times.
 
@@ -45,7 +45,7 @@ def test_umma_fwd_bwd_vs_oracle_at_bench_shapes(d, lmax, lengths, targets, H, dt
     q, k, v, dout, off, nt = _case(d, lmax, lengths, targets, H, dtype, 4242 + d)
     alpha = 1.0 / d**0.5
     qd, kd, vd = (t.to(DEV).requires_grad_() for t in (q, k, v))
-    # d = 256: tcgen05 forward, generic backward (dK + dV alone fill the tensor memory) -> AUTO; otherwise tcgen05 is forced
+    # d = 256: wgmma forward, generic backward (dK + dV alone fill the registers) -> AUTO; otherwise wgmma is forced
     impl = _lib.IMPL_AUTO if d == 256 else _lib.IMPL_UMMA
     if d == 256:
         import ctypes as C
@@ -56,19 +56,19 @@ def test_umma_fwd_bwd_vs_oracle_at_bench_shapes(d, lmax, lengths, targets, H, dt
         _fill_common(p, lmax, alpha, qd, kd, vd, off.to(DEV), nt.to(DEV), 0, 0, 0, _lib.IMPL_AUTO)
         o_ = torch.empty(qd.shape, device=DEV, dtype=dtype)
         p.out, p.o_row_stride, p.o_head_stride = o_.data_ptr(), o_.stride(0), o_.stride(1)
-        assert _lib.lib().hstu_attn_select_impl(C.byref(p), 0) == _lib.IMPL_UMMA, "d = 256 forward must run on tcgen05"
+        assert _lib.lib().hstu_attn_select_impl(C.byref(p), 0) == _lib.IMPL_UMMA, "d = 256 forward must run on wgmma"
     out = hstu_mha(lmax, alpha, qd, kd, vd, off.to(DEV), num_targets=nt.to(DEV), kernel=HammerKernel.CUDA, impl=impl)
     out.backward(dout.to(DEV))
     ref = O.hstu_mha_fwd(lmax, alpha, q, k, v, off, nt)
     rdq, rdk, rdv = O.hstu_mha_bwd(lmax, alpha, dout, q, k, v, off, nt)
     for name, a, r in (("out", out, ref), ("dq", qd.grad, rdq), ("dk", kd.grad, rdk), ("dv", vd.grad, rdv)):
-        assert_rel(a, r, f"tcgen05 d={d} lmax={lmax} {dtype} {name}")
+        assert_rel(a, r, f"wgmma d={d} lmax={lmax} {dtype} {name}")
 
 
 @pytest.mark.parametrize("dout_scale", [1.0, 3e-8, 2e4])
 def test_umma_bwd_is_invariant_to_the_scale_of_dout(dout_scale):
-    """dS is an fp16 operand stored relative to max|dO|: gradients as small as a mean-over-1e7-elements loss produces, or
-    large ones, must come out with the same relative accuracy."""
+    """dS is a 16-bit tensor-core operand: gradients as small as a mean-over-1e7-elements loss produces, or large ones, must
+    come out with the same relative accuracy."""
     from generative_recommenders_b200 import _lib
     from generative_recommenders_b200.common import HammerKernel
     from generative_recommenders_b200.ops.hstu_attention import hstu_mha
@@ -86,7 +86,7 @@ def test_umma_bwd_is_invariant_to_the_scale_of_dout(dout_scale):
 
 
 def test_stu_stack_bf16_gradients_vs_oracle():
-    """The configuration bench.py times -- D=256, H=8, dqk=dv=32, bf16, recompute on, tcgen05 attention writing dq/dk/dv in
+    """The configuration bench.py times -- D=256, H=8, dqk=dv=32, bf16, recompute on, wgmma attention writing dq/dk/dv in
     place into the strided `duvqk` -- forward, dx and EVERY parameter gradient against the fp32 oracle evaluated on the
     bf16-valued parameters.  Between the ops of a layer the GPU path stores bf16 activations (LN output, uvqk, attention
     output, y: ~8 roundings per layer and direction), which the fp32 oracle does not: the budget for this end-to-end

@@ -1,4 +1,4 @@
-"""torch.ops.hstu.hstu_mha / hstu_mha_fwd / hstu_mha_bwd (the reference's native schema, flash_api.cpp:275-365) on B200."""
+"""torch.ops.hstu.hstu_mha / hstu_mha_fwd / hstu_mha_bwd (the reference's native schema, flash_api.cpp:275-365) on H100."""
 import pytest
 import torch
 

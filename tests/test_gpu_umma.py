@@ -1,5 +1,5 @@
-"""GPU: the tcgen05/TMA building blocks (on-device self test) and size-independent properties of the tensor-core
-attention at BASELINE sizes (Lmax up to 8192), where the CPU oracle is too slow to be the checker."""
+"""GPU: the wgmma/TMA building blocks (on-device self test) and size-independent properties of the tensor-core attention at
+BASELINE sizes (Lmax up to 8192), where the CPU oracle is too slow to be the checker."""
 import ctypes as C
 
 import pytest
@@ -41,7 +41,7 @@ def _inputs(B, H, d, lmax, seed, dtype=torch.bfloat16, scale=0.5):
 
 @pytest.mark.parametrize("d,lmax,B,H", [(32, 8192, 2, 8), (64, 2048, 4, 4), (128, 4096, 2, 2), (128, 512, 16, 4)])
 def test_umma_matches_generic_at_full_size(d, lmax, B, H):
-    """Two independent implementations (tcgen05 vs CUDA-core fp32) agree at sizes the CPU oracle cannot reach."""
+    """Two independent implementations (wgmma vs CUDA-core fp32) agree at sizes the CPU oracle cannot reach."""
     from generative_recommenders_b200 import _lib
     from generative_recommenders_b200.common import HammerKernel
     from generative_recommenders_b200.ops.hstu_attention import hstu_mha
@@ -52,7 +52,7 @@ def test_umma_matches_generic_at_full_size(d, lmax, B, H):
                      impl=_lib.IMPL_GENERIC)
     o = hstu_mha(lmax, alpha, q, k, v, off, num_targets=nt, kernel=HammerKernel.CUDA, impl=_lib.IMPL_UMMA)
     assert_rel(o, o_ref, f"umma vs generic d={d} lmax={lmax}")
-    # backward: tcgen05 (where supported) vs the CUDA-core kernels on the same bf16 inputs
+    # backward: wgmma (where supported) vs the CUDA-core kernels on the same bf16 inputs
     do = torch.randn_like(o)
     grads = {}
     for impl in (_lib.IMPL_GENERIC, _lib.IMPL_AUTO):
