@@ -20,6 +20,15 @@
 // P and dS are 16-bit operands of the input format: fp16, or for bf16 inputs a hi + lo pair of bf16 operands (wgmma.cuh,
 // Operand), so that their rounding stays inside the 1e-3 parity budget whatever the scale of dO.
 //
+//
+// d = 32 runs two kernels instead, with no atomics and no coupling between the warpgroups (DESIGN.md 3.2):
+//   attn_bwd_dkdv_wgmma_kernel  the kernel above without the dS buffers, the named barrier and dQ: dK and dV only.
+//   attn_bwd_dq_wgmma_kernel    query-stationary, shaped like the forward: one CTA per (128-row query tile, head, sequence),
+//                               Q and dO resident, K and V streamed in 64-key tiles; it recomputes S = Q K^T and
+//                               dP = dO V^T, forms dS from one tanh and accumulates dQ += dS K in registers.
+// At d = 32 recomputing S and dP costs two MMA units per score against the eight that the whole backward issues, while the
+// elementwise work per score is the same; at larger d the recomputed MMAs weigh more and the fused kernel is kept.
+//
 // Reference math: ops/triton/triton_hstu_attention.py:995-1006,1222 and SURVEY.md appendix A; unlike the Triton
 // kernel dQ is accumulated in fp32, not in the input dtype (triton_attention_utils.py:47-60).
 #include <string.h>
@@ -40,8 +49,9 @@ struct alignas(64) BwdParams {
   const void* num_targets;
   void* dk;
   void* dv;
-  float* dq_acc;  // [L, H, D] fp32, zero-initialised
-  long long dk_row_stride, dk_head_stride, dv_row_stride, dv_head_stride;
+  float* dq_acc;  // [L, H, D] fp32, zero-initialised (fused kernel)
+  void* dq;       // attn_bwd_dq_wgmma_kernel
+  long long dk_row_stride, dk_head_stride, dv_row_stride, dv_head_stride, dq_row_stride, dq_head_stride;
   int offsets_i64, targets_i64;
   int max_seq_len, heads;
   int win, min_full, ctx;
@@ -50,7 +60,8 @@ struct alignas(64) BwdParams {
   float dk_scale;  // alpha / (2 N): dS^T holds 2 dS N / alpha
 };
 
-template <int D>
+// FUSED_DQ: the key-tile kernel also computes dQ (dS buffers in shared memory); without it the layout ends after the ring
+template <int D, bool FUSED_DQ = true>
 struct BwdCfg {
   static constexpr int BKV = 128, BQ = 64;
   static constexpr int SW = (D * 2 >= 128) ? 128 : D * 2;
@@ -68,7 +79,7 @@ struct BwdCfg {
   static constexpr int OFF_Q = OFF_V + KV_BYTES;
   static constexpr int OFF_DO = OFF_Q + STAGES * QD_BYTES;
   static constexpr int OFF_DS = OFF_DO + STAGES * QD_BYTES;          // [buffer 0/1][hi / lo]
-  static constexpr int OFF_BAR = OFF_DS + 4 * DS_BYTES;
+  static constexpr int OFF_BAR = OFF_DS + (FUSED_DQ ? 4 * DS_BYTES : 0);
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
@@ -85,9 +96,11 @@ struct QTiles {
   __device__ __forceinline__ int at(int i) const { return i < A ? i : first + (i - A); }
 };
 
-template <int D, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __grid_constant__ BwdParams p) {
-  using Cfg = BwdCfg<D>;
+// Body of the key-stationary kernels: FUSED_DQ = attn_bwd_wgmma_kernel (dK, dV and the dQ atomics), otherwise
+// attn_bwd_dkdv_wgmma_kernel (dK and dV only; the warpgroups meet only at the ring's empty barriers).
+template <int D, bool BF16, bool FUSED_DQ>
+__device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
+  using Cfg = BwdCfg<D, FUSED_DQ>;
   constexpr int SW = Cfg::SW, BQ = Cfg::BQ, NST = Cfg::STAGES;
   const int b = blockIdx.z, h = blockIdx.y;
   const int n0 = blockIdx.x * Cfg::BKV;
@@ -217,26 +230,60 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __
         s[nb * 4 + e] = pv;
         dp[nb * 4 + e] = dsv;
       }
+    if constexpr (FUSED_DQ) {
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
+      for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const Operand<BF16> pp(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]), dd(dp[8 * kk + 2 * r], dp[8 * kk + 2 * r + 1]);
-        pf_hi[kk][r] = pp.hi; pf_lo[kk][r] = pp.lo;
-        df_hi[kk][r] = dd.hi; df_lo[kk][r] = dd.lo;
+        for (int r = 0; r < 4; ++r) {
+          const Operand<BF16> pp(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]), dd(dp[8 * kk + 2 * r], dp[8 * kk + 2 * r + 1]);
+          pf_hi[kk][r] = pp.hi; pf_lo[kk][r] = pp.lo;
+          df_hi[kk][r] = dd.hi; df_lo[kk][r] = dd.lo;
+        }
       }
-    }
-    // dV += P^T dO_j, dK += dS^T Q_j
-    wgmma_fence();
+      // dV += P^T dO_j, dK += dS^T Q_j
+      wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const uint64_t dod = desc_mnmajor<SW>(sdo + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
-      const uint64_t qd = desc_mnmajor<SW>(sq + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
-      wgmma_rs<D, BF16, 1>(dv, pf_hi[kk], dod, 1);
-      wgmma_rs<D, BF16, 1>(dk, df_hi[kk], qd, 1);
-      if constexpr (BF16) {
-        wgmma_rs<D, BF16, 1>(dv, pf_lo[kk], dod, 1);
-        wgmma_rs<D, BF16, 1>(dk, df_lo[kk], qd, 1);
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t dod = desc_mnmajor<SW>(sdo + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
+        const uint64_t qd = desc_mnmajor<SW>(sq + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
+        wgmma_rs<D, BF16, 1>(dv, pf_hi[kk], dod, 1);
+        wgmma_rs<D, BF16, 1>(dk, df_hi[kk], qd, 1);
+        if constexpr (BF16) {
+          wgmma_rs<D, BF16, 1>(dv, pf_lo[kk], dod, 1);
+          wgmma_rs<D, BF16, 1>(dk, df_lo[kk], qd, 1);
+        }
+      }
+    } else {
+      // dV += P^T dO_j issued as soon as P is packed, then dK += dS^T Q_j: P^T and dS^T are never both held in fp32 next to
+      // both fragment sets, which keeps a bf16 thread at 128 registers without wgmma serialisation (ptxas C7512)
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const Operand<BF16> pp(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+          pf_hi[kk][r] = pp.hi; pf_lo[kk][r] = pp.lo;
+        }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t dod = desc_mnmajor<SW>(sdo + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
+        wgmma_rs<D, BF16, 1>(dv, pf_hi[kk], dod, 1);
+        if constexpr (BF16) wgmma_rs<D, BF16, 1>(dv, pf_lo[kk], dod, 1);
+      }
+      wgmma_commit();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const Operand<BF16> dd(dp[8 * kk + 2 * r], dp[8 * kk + 2 * r + 1]);
+          df_hi[kk][r] = dd.hi; df_lo[kk][r] = dd.lo;
+        }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t qd = desc_mnmajor<SW>(sq + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
+        wgmma_rs<D, BF16, 1>(dk, df_hi[kk], qd, 1);
+        if constexpr (BF16) wgmma_rs<D, BF16, 1>(dk, df_lo[kk], qd, 1);
       }
     }
     wgmma_commit();
@@ -250,6 +297,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __
     mbar_arrive(&bars->qd_empty[st]);
     if (tid == 0 && j + NST < qt.T) load_qd(j + NST);  // Q_j and dO_j are no longer read
     __syncwarp();
+    if constexpr (!FUSED_DQ) continue;
     // dS^T -> shared memory buffer j & 1: element (kv r, q c) of a [128][64] 16-bit box with 128-byte swizzle
     const uint32_t dsb = sds + (j & 1) * 2 * Cfg::DS_BYTES;
 #pragma unroll
@@ -311,6 +359,213 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __
   }
 }
 
+template <int D, bool BF16>
+__global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __grid_constant__ BwdParams p) {
+  bwd_key_tile<D, BF16, true>(p);
+}
+
+// two CTAs per SM (<= 128 registers per thread, 49 KB of shared memory at d = 32)
+template <int D, bool BF16>
+__global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dkdv_wgmma_kernel(const __grid_constant__ BwdParams p) {
+  bwd_key_tile<D, BF16, false>(p);
+}
+
+// ---------------- dQ, query-stationary (d = 32) ----------------
+template <int D>
+struct DqCfg {
+  static constexpr int BM = 128;  // query rows per CTA (two warpgroups of 64)
+  static constexpr int BN = 64;   // key rows per tile
+  static constexpr int SW = (D * 2 >= 128) ? 128 : D * 2;
+  static constexpr int BOX_COLS = SW / 2;
+  static constexpr int NBOX = D / BOX_COLS;
+  static constexpr int Q_BOX = BM * SW;
+  static constexpr int KV_BOX = BN * SW;
+  static constexpr int Q_BYTES = BM * D * 2;
+  static constexpr int KV_BYTES = BN * D * 2;
+  static constexpr int STAGES = 3;  // K / V ring depth
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_DO = OFF_Q + Q_BYTES;
+  static constexpr int OFF_K = OFF_DO + Q_BYTES;
+  static constexpr int OFF_V = OFF_K + STAGES * KV_BYTES;
+  static constexpr int OFF_BAR = OFF_V + STAGES * KV_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+  static_assert(SMEM_BYTES <= 232448 / 2, "shared memory budget of two CTAs per SM");
+};
+
+struct DqBars {
+  uint64_t qd_full;
+  uint64_t k_full[3], v_full[3], k_empty[3], v_empty[3];
+};
+
+// One CTA per (128-row query tile, head, sequence), heavy (late) tiles first; the forward's schedule, tile ranges and ring.
+// Per 64-key tile each warpgroup runs S = Q K^T and dP = dO V^T (A and B K-major), releases V, forms
+// 2 dS N / alpha = dP (1 + g2) * mask from one tanh, and runs dQ += dS K (A from registers, K read MN-major), then releases K.
+template <int D, bool BF16>
+__global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const __grid_constant__ BwdParams p) {
+  using Cfg = DqCfg<D>;
+  constexpr int SW = Cfg::SW, BN = Cfg::BN, NST = Cfg::STAGES;
+  const int b = blockIdx.z, h = blockIdx.y;
+  const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
+  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
+  int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
+  if (len > p.max_seq_len) {  // rows past max_seq_len get zero gradients
+    if (blockIdx.x == 0) zero_rows(p.dq, 2, p.dq_row_stride, (long long)h * p.dq_head_stride, D, row0 + p.max_seq_len, row0 + len);
+    len = p.max_seq_len;
+  }
+  if (m0 >= len) return;
+  const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
+  const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
+  const int mrows = min(Cfg::BM, len - m0);
+  int lo, hi;
+  kv_range_for_q_rows(msk, m0, m0 + mrows, &lo, &hi);
+  const int t0 = lo / BN;
+  const int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  DqBars* bars = reinterpret_cast<DqBars*>(smem + Cfg::OFF_BAR);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    mbar_init(&bars->qd_full, 1);
+    for (int i = 0; i < NST; ++i) {
+      mbar_init(&bars->k_full[i], 1);
+      mbar_init(&bars->v_full[i], 1);
+      mbar_init(&bars->k_empty[i], 256);
+      mbar_init(&bars->v_empty[i], 256);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  // TMA issue (thread 0): Q, dO and the first STAGES key tiles now; stage st is refilled once both warpgroups have released
+  // its V (after S / dP) and its K (after dQ)
+  auto load_kv = [&](int i) {
+    const int st = i % NST;
+    const int kv_row = (int)(row0 + (long long)(t0 + i) * BN);
+    if (i >= NST) mbar_wait(&bars->k_empty[st], ((i / NST) - 1) & 1);
+    mbar_arrive_expect_tx(&bars->k_full[st], Cfg::KV_BYTES);
+#pragma unroll
+    for (int bx = 0; bx < Cfg::NBOX; ++bx)
+      tma_load_3d(smem + Cfg::OFF_K + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmK, &bars->k_full[st], bx * Cfg::BOX_COLS, h, kv_row);
+    if (i >= NST) mbar_wait(&bars->v_empty[st], ((i / NST) - 1) & 1);
+    mbar_arrive_expect_tx(&bars->v_full[st], Cfg::KV_BYTES);
+#pragma unroll
+    for (int bx = 0; bx < Cfg::NBOX; ++bx)
+      tma_load_3d(smem + Cfg::OFF_V + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmV, &bars->v_full[st], bx * Cfg::BOX_COLS, h, kv_row);
+  };
+  if (tid == 0) {
+    prefetch_tensormap(&p.tmQ);
+    prefetch_tensormap(&p.tmK);
+    prefetch_tensormap(&p.tmV);
+    prefetch_tensormap(&p.tmDO);
+    mbar_arrive_expect_tx(&bars->qd_full, 2 * Cfg::Q_BYTES);
+#pragma unroll
+    for (int bx = 0; bx < Cfg::NBOX; ++bx) {
+      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->qd_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
+      tma_load_3d(smem + Cfg::OFF_DO + bx * Cfg::Q_BOX, &p.tmDO, &bars->qd_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
+    }
+    for (int i = 0; i < min(T, NST); ++i) load_kv(i);
+  }
+  __syncwarp();
+
+  const int wgi = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
+  const int q_base = m0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
+  const uint32_t sq = smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW, sdo = smem_u32(smem + Cfg::OFF_DO) + wgi * 64 * SW;
+  const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
+  const bool fast = msk.fast != 0;
+  const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
+
+  float dq[D / 2];
+#pragma unroll
+  for (int e = 0; e < D / 2; ++e) dq[e] = 0.f;
+  uint32_t a_hi[BN / 16][4], a_lo[BN / 16][4];
+#pragma unroll
+  for (int kk = 0; kk < BN / 16; ++kk)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) a_hi[kk][r] = a_lo[kk][r] = 0u;
+  mbar_wait(&bars->qd_full, 0);
+  for (int i = 0; i < T; ++i) {
+    const int st = i % NST;
+    const uint32_t ph = (i / NST) & 1;
+    const uint32_t kst = sk + st * Cfg::KV_BYTES, vst = sv + st * Cfg::KV_BYTES;
+    float s[BN / 2], dp[BN / 2];
+    mbar_wait(&bars->k_full[st], ph);
+    mbar_wait(&bars->v_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < D / 16; ++ks) {
+      const int kb = ks * 32, bx = kb / SW, off = kb % SW;
+      wgmma_ss<BN, BF16, 0, 0>(s, desc_kmajor<SW>(sq + bx * Cfg::Q_BOX, off), desc_kmajor<SW>(kst + bx * Cfg::KV_BOX, off), ks > 0);
+    }
+#pragma unroll
+    for (int ks = 0; ks < D / 16; ++ks) {
+      const int kb = ks * 32, bx = kb / SW, off = kb % SW;
+      wgmma_ss<BN, BF16, 0, 0>(dp, desc_kmajor<SW>(sdo + bx * Cfg::Q_BOX, off), desc_kmajor<SW>(vst + bx * Cfg::KV_BOX, off), ks > 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    fence_regs(dp);
+    mbar_arrive(&bars->v_empty[st]);
+
+    // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2
+    const int n0 = (t0 + i) * BN;
+    const bool full = n0 + BN <= full_lim;  // tile-uniform
+#pragma unroll
+    for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float x = s[nb * 4 + e] * p.alpha_half;
+        const float t = tanh_approx(x);
+        const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
+        float dsv = __fmaf_rn(dp[nb * 4 + e], g2, dp[nb * 4 + e]);
+        if (!full) {
+          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+          dsv = (kj < len && mask_valid(msk, qi, kj)) ? dsv : 0.f;
+        }
+        dp[nb * 4 + e] = dsv;
+      }
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; ++kk) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const Operand<BF16> x(dp[8 * kk + 2 * r], dp[8 * kk + 2 * r + 1]);
+        a_hi[kk][r] = x.hi;
+        a_lo[kk][r] = x.lo;
+      }
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; ++kk) {
+      const uint64_t kd = desc_mnmajor<SW>(kst, kk * 16, Cfg::KV_BOX);
+      wgmma_rs<D, BF16, 1>(dq, a_hi[kk], kd, 1);
+      if constexpr (BF16) wgmma_rs<D, BF16, 1>(dq, a_lo[kk], kd, 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();  // an MMA batch never stays in flight across the elementwise code (ptxas would serialise them)
+    fence_regs(dq);
+    fence_regs(a_hi);
+    fence_regs(a_lo);
+    mbar_arrive(&bars->k_empty[st]);
+    if (tid == 0 && i + NST < T) load_kv(i + NST);  // K and V of tile i are no longer read
+    __syncwarp();
+  }
+
+  // ---------------- epilogue: dQ * alpha / (2N) -> global ----------------
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int qi = q_base + hh * 8;
+    if (qi - m0 < mrows) {
+      uint16_t* qrow = reinterpret_cast<uint16_t*>(p.dq) + (row0 + qi) * p.dq_row_stride + (long long)h * p.dq_head_stride;
+#pragma unroll
+      for (int nb = 0; nb < D / 8; ++nb) {
+        const float a = dq[nb * 4 + hh * 2] * p.dk_scale, c = dq[nb * 4 + hh * 2 + 1] * p.dk_scale;
+        *reinterpret_cast<uint32_t*>(qrow + nb * 8 + 2 * t4) = BF16 ? pack_bf16x2(a, c) : pack_f16x2(a, c);
+      }
+    }
+  }
+}
+
 // dq[r, h, :] = convert(dq_acc[r, h, :] * scale)
 template <bool BF16>
 __global__ void dq_convert_kernel(const float* __restrict__ acc, uint16_t* __restrict__ dq, long long rows, int heads, int D,
@@ -355,16 +610,20 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd) {
   return wgmma_bwd_supported(q);
 }
 
+// d = 32: dK / dV and dQ in two kernels, without atomics or workspace; larger d: the fused kernel (DESIGN.md 3.2)
+static constexpr bool split_dq(int d) { return d == 32; }
+
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd) {
-  if (!bwd) return 0;
+  if (!bwd || split_dq(p.dqk)) return 0;
   return (size_t)p.total_rows * p.heads * p.dqk * sizeof(float);  // fp32 dQ accumulator [L, H, D]
 }
 
 template <int D, bool BF16>
 static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
-  using Cfg = BwdCfg<D>;
+  constexpr bool kSplit = split_dq(D);
+  using Cfg = BwdCfg<D, !kSplit>;
   const size_t need = wgmma_workspace_bytes(p, true);
-  if (p.workspace == nullptr || p.workspace_bytes < need) {
+  if (need > 0 && (p.workspace == nullptr || p.workspace_bytes < need)) {
     set_error("hstu_attn_bwd: workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
     return HSTU_ERR_WORKSPACE;
   }
@@ -379,10 +638,13 @@ static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
   bp.dk = p.dk;
   bp.dv = p.dv_out;
   bp.dq_acc = reinterpret_cast<float*>(p.workspace);
+  bp.dq = p.dq;
   bp.dk_row_stride = p.dk_row_stride;
   bp.dk_head_stride = p.dk_head_stride;
   bp.dv_row_stride = p.dv_row_stride;
   bp.dv_head_stride = p.dv_head_stride;
+  bp.dq_row_stride = p.dq_row_stride;
+  bp.dq_head_stride = p.dq_head_stride;
   bp.offsets_i64 = p.offsets_are_i64;
   bp.targets_i64 = p.num_targets_are_i64;
   bp.max_seq_len = p.max_seq_len;
@@ -393,18 +655,35 @@ static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
   bp.alpha_half = 0.5f * p.alpha;
   bp.dv_scale = 1.0f / (float)p.max_seq_len;
   bp.dk_scale = 0.5f * p.alpha / (float)p.max_seq_len;
-  HSTU_CUDA_OK(cudaMemsetAsync(p.workspace, 0, need, st));
-  auto kern = attn_bwd_wgmma_kernel<D, BF16>;
-  HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  dim3 grid((p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV, p.heads, p.batch);
-  kern<<<grid, kBwdThreads, Cfg::SMEM_BYTES, st>>>(bp);
-  HSTU_CUDA_OK(cudaGetLastError());
-  const long long nvec = p.total_rows * p.heads * (D / 8);
-  long long blocks = (nvec + 255) / 256;
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  dq_convert_kernel<BF16><<<(int)blocks, 256, 0, st>>>(bp.dq_acc, reinterpret_cast<uint16_t*>(p.dq), p.total_rows, p.heads, D,
-                                                       p.dq_row_stride, p.dq_head_stride, bp.dk_scale);
-  HSTU_CUDA_OK(cudaGetLastError());
+  if constexpr (kSplit) {
+    auto kdkdv = attn_bwd_dkdv_wgmma_kernel<D, BF16>;
+    HSTU_CUDA_OK(cudaFuncSetAttribute(kdkdv, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    kdkdv<<<dim3((p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV, p.heads, p.batch), kBwdThreads, Cfg::SMEM_BYTES, st>>>(bp);
+    HSTU_CUDA_OK(cudaGetLastError());
+    // the dQ kernel tiles 128 query rows and 64 key rows
+    using QC = DqCfg<D>;
+    if (int e = make_tmap_rows_heads(&bp.tmQ, p.q, p.total_rows, p.heads, D, p.q_row_stride, p.q_head_stride, QC::BOX_COLS, QC::BM)) return e;
+    if (int e = make_tmap_rows_heads(&bp.tmK, p.k, p.total_rows, p.heads, D, p.k_row_stride, p.k_head_stride, QC::BOX_COLS, QC::BN)) return e;
+    if (int e = make_tmap_rows_heads(&bp.tmV, p.v, p.total_rows, p.heads, D, p.v_row_stride, p.v_head_stride, QC::BOX_COLS, QC::BN)) return e;
+    if (int e = make_tmap_rows_heads(&bp.tmDO, p.dout, p.total_rows, p.heads, D, p.do_row_stride, p.do_head_stride, QC::BOX_COLS, QC::BM)) return e;
+    auto kdq = attn_bwd_dq_wgmma_kernel<D, BF16>;
+    HSTU_CUDA_OK(cudaFuncSetAttribute(kdq, cudaFuncAttributeMaxDynamicSharedMemorySize, QC::SMEM_BYTES));
+    kdq<<<dim3((p.max_seq_len + QC::BM - 1) / QC::BM, p.heads, p.batch), kBwdThreads, QC::SMEM_BYTES, st>>>(bp);
+    HSTU_CUDA_OK(cudaGetLastError());
+  } else {
+    HSTU_CUDA_OK(cudaMemsetAsync(p.workspace, 0, need, st));
+    auto kern = attn_bwd_wgmma_kernel<D, BF16>;
+    HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    dim3 grid((p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV, p.heads, p.batch);
+    kern<<<grid, kBwdThreads, Cfg::SMEM_BYTES, st>>>(bp);
+    HSTU_CUDA_OK(cudaGetLastError());
+    const long long nvec = p.total_rows * p.heads * (D / 8);
+    long long blocks = (nvec + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    dq_convert_kernel<BF16><<<(int)blocks, 256, 0, st>>>(bp.dq_acc, reinterpret_cast<uint16_t*>(p.dq), p.total_rows, p.heads, D,
+                                                         p.dq_row_stride, p.dq_head_stride, bp.dk_scale);
+    HSTU_CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }
 

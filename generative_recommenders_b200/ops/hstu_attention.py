@@ -116,7 +116,7 @@ def cuda_hstu_attention_bwd(
     ws = _workspace(p, True, dev)
     with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
         _lib.check(_lib.lib().hstu_attn_bwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_bwd")
-    # wgmma path: main kernel + dQ convert; generic path: dK/dV kernel + dQ kernel
+    # wgmma path: dK/dV kernel + dQ kernel (d = 32) or main kernel + dQ convert; generic path: dK/dV kernel + dQ kernel
     _lib.note_launch(2)
     del ws, keep
 

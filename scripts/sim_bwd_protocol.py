@@ -129,6 +129,40 @@ def run(T, d, seed, break_ds=False):
     return _simulate({"W0": W(0), "W1": W(1)}, B, rnd)
 
 
+DKDV_STAGES = 4  # BwdCfg<32, false>::STAGES
+
+
+def run_dkdv(T, seed, break_release=False):
+    """attn_bwd_dkdv_wgmma_kernel (d = 32): the key-tile CTA of `run` without dS buffers, named barrier or dQ; the two
+    warpgroups meet only at the Q / dO empty barriers.  break_release: thread 0 refills a stage once its own warpgroup has
+    released it, without waiting for the other one (must be caught)."""
+    NST = DKDV_STAGES
+    rnd = random.Random(seed)
+    B = {"kv": Bar(1)}
+    for i in range(NST):
+        B[f"qf{i}"] = Bar(1)
+        B[f"qe{i}"] = Bar(2)
+
+    def W(w):
+        if w == 0:
+            yield ("async", "kv")
+            for j in range(min(T, NST)):
+                yield ("tma", f"qf{j % NST}", f"q{j % NST}")
+        yield ("wait", "kv", 0)
+        for j in range(T):
+            st = j % NST
+            yield ("wait", f"qf{st}", j // NST)
+            yield ("read", f"q{st}", 1)              # S^T, dP^T, dV, dK MMAs, waited for
+            yield ("read", f"q{st}", -1)
+            yield ("arrive", f"qe{st}")
+            if w == 0 and j + NST < T:
+                if not break_release:
+                    yield ("wait", f"qe{st}", j // NST)
+                yield ("tma", f"qf{st}", f"q{st}")
+
+    return _simulate({"W0": W(0), "W1": W(1)}, B, rnd)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--d", type=int, default=32, choices=sorted(STAGES))

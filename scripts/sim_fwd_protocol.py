@@ -60,6 +60,53 @@ def run(T, d, seed, break_refill=False):
     return _eng._simulate({"W0": W(0), "W1": W(1)}, B, rnd)
 
 
+DQ_STAGES = 3  # DqCfg<32>::STAGES (csrc/attn_wgmma_bwd.cu)
+
+
+def run_dq(T, seed, break_k_refill=False):
+    """attn_bwd_dq_wgmma_kernel (d = 32): the forward's ring with Q and dO resident; S / dP read K and V, V is released,
+    then dQ += dS K reads K, and K is released.  break_k_refill: the K refill waits for the release of V instead of K, i.e.
+    it may land while the other warpgroup's dQ MMA still reads K (must be caught)."""
+    NST = DQ_STAGES
+    rnd = random.Random(seed)
+    B = {"qd": Bar(1)}
+    for i in range(NST):
+        B[f"kf{i}"], B[f"vf{i}"] = Bar(1), Bar(1)
+        B[f"ke{i}"], B[f"ve{i}"] = Bar(2), Bar(2)
+
+    def load(i):
+        st = i % NST
+        if i >= NST:
+            yield ("wait", f"{'ve' if break_k_refill else 'ke'}{st}", i // NST - 1)
+        yield ("tma", f"kf{st}", f"k{st}")
+        if i >= NST:
+            yield ("wait", f"ve{st}", i // NST - 1)
+        yield ("tma", f"vf{st}", f"v{st}")
+
+    def W(w):
+        if w == 0:
+            yield ("async", "qd")
+            for i in range(min(T, NST)):
+                yield from load(i)
+        yield ("wait", "qd", 0)
+        for i in range(T):
+            st = i % NST
+            yield ("wait", f"kf{st}", i // NST)
+            yield ("wait", f"vf{st}", i // NST)
+            yield ("read", f"k{st}", 1)          # S = Q K^T and dP = dO V^T, waited for
+            yield ("read", f"v{st}", 1)
+            yield ("read", f"v{st}", -1)
+            yield ("arrive", f"ve{st}")
+            yield ("read", f"k{st}", -1)
+            yield ("read", f"k{st}", 1)          # dQ += dS K, waited for
+            yield ("read", f"k{st}", -1)
+            yield ("arrive", f"ke{st}")
+            if w == 0 and i + NST < T:
+                yield from load(i + NST)
+
+    return _eng._simulate({"W0": W(0), "W1": W(1)}, B, rnd)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--d", type=int, default=32, choices=sorted(STAGES))
