@@ -12,8 +12,9 @@
 //                    computes dQ_j = dS K over all 128 keys (A = dS^T MN-major, B = K MN-major) and adds it to an fp32
 //                    accumulator in global memory (each key-tile CTA contributes to every later query tile); a small convert
 //                    kernel scales it by alpha/N and writes dq in the input dtype.
-// Thread 0 issues the TMA loads: K and V once, then Q_j and dO_j; a stage is refilled once all 256 threads have released it
-// (the MMAs that read it have completed).  No separate producer warp: the dK and dV accumulators (d = 128: 64 registers each
+// Thread 0 issues the first TMA loads: K and V once, then Q_j and dO_j; afterwards each warp releases a stage once its MMAs
+// that read it have completed, and the warp whose release is the last of the eight refills it (release_is_last, wgmma.cuh),
+// so no thread waits for a free stage.  No separate producer warp: the dK and dV accumulators (d = 128: 64 registers each
 // per thread) need the register budget of a 256-thread block.
 // Each warpgroup waits for its own MMAs before the next elementwise step (an MMA batch left in flight across it makes ptxas
 // serialise the batch); a Q_j / dO_j stage is released as soon as dV / dK of tile j have completed.
@@ -25,7 +26,8 @@
 //   attn_bwd_dkdv_wgmma_kernel  the kernel above without the dS buffers, the named barrier and dQ: dK and dV only.
 //   attn_bwd_dq_wgmma_kernel    query-stationary, shaped like the forward: one CTA per (128-row query tile, head, sequence),
 //                               Q and dO resident, K and V streamed in 64-key tiles; it recomputes S = Q K^T and
-//                               dP = dO V^T, forms dS from one tanh and accumulates dQ += dS K in registers.
+//                               dP = dO V^T, forms dS from one tanh and accumulates dQ += dS K in registers.  Its K / V ring
+//                               is refilled like the forward's, by the last warp to release a stage.
 // At d = 32 recomputing S and dP costs two MMA units per score against the eight that the whole backward issues, while the
 // elementwise work per score is the same; at larger d the recomputed MMAs weigh more and the fused kernel is kept.
 //
@@ -87,7 +89,8 @@ constexpr int kBwdThreads = 256;
 
 struct BwdBars {
   uint64_t kv_full;
-  uint64_t qd_full[4], qd_empty[4];
+  uint64_t qd_full[4];
+  uint32_t qd_free[4];  // release counters of the Q_j / dO_j stages (release_is_last: one arrival per warp and use)
 };
 
 // query tiles of a key tile: the contextual prefix tiles [0, A), then the causal / window range
@@ -134,17 +137,17 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     mbar_init(&bars->kv_full, 1);
     for (int i = 0; i < NST; ++i) {
       mbar_init(&bars->qd_full[i], 1);
-      mbar_init(&bars->qd_empty[i], 256);
+      bars->qd_free[i] = 0u;
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  // TMA issue (thread 0): K, V and the first STAGES query tiles now; stage st is refilled once both warpgroups have released it
+  // TMA issue: thread 0 loads K, V and the first STAGES query tiles; the warp that completes the release of a stage (below)
+  // loads query tile j + STAGES into it
   auto load_qd = [&](int j) {
     const int st = j % NST;
     const int q_row = (int)(row0 + (long long)qt.at(j) * BQ);
-    if (j >= NST) mbar_wait(&bars->qd_empty[st], ((j / NST) - 1) & 1);
     mbar_arrive_expect_tx(&bars->qd_full[st], 2 * Cfg::QD_BYTES);
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx) {
@@ -294,8 +297,8 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     fence_regs(pf_lo);
     fence_regs(df_hi);
     fence_regs(df_lo);
-    mbar_arrive(&bars->qd_empty[st]);
-    if (tid == 0 && j + NST < qt.T) load_qd(j + NST);  // Q_j and dO_j are no longer read
+    // Q_j and dO_j are no longer read by this warp; the last of the eight warps to say so refills the stage
+    if (lane == 0 && j + NST < qt.T && release_is_last<kBwdThreads / 32>(&bars->qd_free[st])) load_qd(j + NST);
     __syncwarp();
     if constexpr (!FUSED_DQ) continue;
     // dS^T -> shared memory buffer j & 1: element (kv r, q c) of a [128][64] 16-bit box with 128-byte swizzle
@@ -394,7 +397,8 @@ struct DqCfg {
 
 struct DqBars {
   uint64_t qd_full;
-  uint64_t k_full[3], v_full[3], k_empty[3], v_empty[3];
+  uint64_t k_full[3], v_full[3];
+  uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
 };
 
 // One CTA per (128-row query tile, head, sequence), heavy (late) tiles first; the forward's schedule, tile ranges and ring.
@@ -430,28 +434,26 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
     for (int i = 0; i < NST; ++i) {
       mbar_init(&bars->k_full[i], 1);
       mbar_init(&bars->v_full[i], 1);
-      mbar_init(&bars->k_empty[i], 256);
-      mbar_init(&bars->v_empty[i], 256);
+      bars->k_free[i] = bars->v_free[i] = 0u;
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  // TMA issue (thread 0): Q, dO and the first STAGES key tiles now; stage st is refilled once both warpgroups have released
-  // its V (after S / dP) and its K (after dQ)
-  auto load_kv = [&](int i) {
+  // TMA issue of key tile i into its K or V stage (tm = &p.tmK / &p.tmV, off = Cfg::OFF_K / OFF_V, full = its full barriers)
+  auto load = [&](const CUtensorMap* tm, int off, uint64_t* full, int i) {
     const int st = i % NST;
-    const int kv_row = (int)(row0 + (long long)(t0 + i) * BN);
-    if (i >= NST) mbar_wait(&bars->k_empty[st], ((i / NST) - 1) & 1);
-    mbar_arrive_expect_tx(&bars->k_full[st], Cfg::KV_BYTES);
+    mbar_arrive_expect_tx(&full[st], Cfg::KV_BYTES);
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx)
-      tma_load_3d(smem + Cfg::OFF_K + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmK, &bars->k_full[st], bx * Cfg::BOX_COLS, h, kv_row);
-    if (i >= NST) mbar_wait(&bars->v_empty[st], ((i / NST) - 1) & 1);
-    mbar_arrive_expect_tx(&bars->v_full[st], Cfg::KV_BYTES);
-#pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX; ++bx)
-      tma_load_3d(smem + Cfg::OFF_V + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmV, &bars->v_full[st], bx * Cfg::BOX_COLS, h, kv_row);
+      tma_load_3d(smem + off + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, tm, &full[st], bx * Cfg::BOX_COLS, h,
+                  (int)(row0 + (long long)(t0 + i) * BN));
+  };
+  // Thread 0 loads Q, dO and the first STAGES key tiles.  Afterwards each warp releases the V stage of tile i once its S / dP
+  // MMAs have completed and the K stage once its dQ MMAs have, and the warp whose release is the last of the eight loads tile
+  // i + STAGES into the stage (the forward's protocol).
+  auto release = [&](const CUtensorMap* tm, int off, uint64_t* full, uint32_t* ctr, int i) {
+    if (lane == 0 && i + NST < T && release_is_last<kBwdThreads / 32>(&ctr[i % NST])) load(tm, off, full, i + NST);
   };
   if (tid == 0) {
     prefetch_tensormap(&p.tmQ);
@@ -464,7 +466,10 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
       tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->qd_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
       tma_load_3d(smem + Cfg::OFF_DO + bx * Cfg::Q_BOX, &p.tmDO, &bars->qd_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
     }
-    for (int i = 0; i < min(T, NST); ++i) load_kv(i);
+    for (int i = 0; i < min(T, NST); ++i) {
+      load(&p.tmK, Cfg::OFF_K, bars->k_full, i);
+      load(&p.tmV, Cfg::OFF_V, bars->v_full, i);
+    }
   }
   __syncwarp();
 
@@ -483,6 +488,8 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
   for (int kk = 0; kk < BN / 16; ++kk)
 #pragma unroll
     for (int r = 0; r < 4; ++r) a_hi[kk][r] = a_lo[kk][r] = 0u;
+  // One wait per MMA batch: S and dP of tile i + 1 in the batch of dQ += dS_i K_i would hold S, dP, dQ and both dS fragment
+  // sets at once, which does not fit in 128 registers with bf16 inputs (ptxas spills and serialises the MMAs).
   mbar_wait(&bars->qd_full, 0);
   for (int i = 0; i < T; ++i) {
     const int st = i % NST;
@@ -506,7 +513,8 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
     wgmma_wait<0>();
     fence_regs(s);
     fence_regs(dp);
-    mbar_arrive(&bars->v_empty[st]);
+    release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i);
+    __syncwarp();
 
     // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2
     const int n0 = (t0 + i) * BN;
@@ -546,8 +554,7 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
     fence_regs(dq);
     fence_regs(a_hi);
     fence_regs(a_lo);
-    mbar_arrive(&bars->k_empty[st]);
-    if (tid == 0 && i + NST < T) load_kv(i + NST);  // K and V of tile i are no longer read
+    release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i);
     __syncwarp();
   }
 

@@ -7,10 +7,13 @@
 //   P = silu(alpha S) * mask   (one tanh per score, in registers)
 //   O += P V             (wgmma, A = P from registers, B = V MN-major in shared memory)
 // Key tiles of 64 rows keep a thread at <= 128 registers for d <= 64, so two CTAs share an SM there.
-// Each warpgroup waits for its own MMAs; the two warpgroups overlap each other's tensor-core and elementwise phases.
-// Thread 0 issues the TMA loads: Q once, then the K and V tiles through a ring of STAGES buffers each; a stage is refilled
-// once all 256 threads have released it (the MMAs that read it have completed).  No separate producer warp: the 64 x d
-// fp32 O accumulator (d = 256: 128 registers per thread) needs the register budget of a 256-thread block.
+// Each warpgroup waits for its own MMAs; the two warpgroups overlap each other's tensor-core and elementwise phases.  With
+// d <= 64, O += P_i V_i and S_{i+1} = Q K_{i+1}^T are one MMA batch with one wait per tile (O is never read in the loop).
+// Thread 0 issues the first TMA loads: Q, then the K and V tiles through a ring of STAGES buffers each.  Each warp releases a
+// stage once its MMAs that read it have completed, and the warp whose release is the last of the eight issues the refill
+// (release_is_last, wgmma.cuh), so no thread ever waits for a free stage and neither warpgroup holds the other back.  No
+// separate producer warp: the 64 x d fp32 O accumulator (d = 256: 128 registers per thread) needs the register budget of a
+// 256-thread block.
 // P is a 16-bit MMA operand of the same format as V (wgmma takes one format for A and B): fp16 for fp16 inputs, and for
 // bf16 inputs a hi + lo pair of bf16 operands multiplied twice (wgmma.cuh, Operand), so that its rounding stays well inside
 // the 1e-3 parity budget.  The 1/N factor of the reference is applied once in the epilogue (registers -> global, rows past
@@ -64,13 +67,17 @@ template <int D> constexpr int kFwdMinBlocks = (D <= 64) ? 2 : 1;  // d <= 64: t
 
 struct FwdBars {
   uint64_t q_full;
-  uint64_t k_full[3], v_full[3], k_empty[3], v_empty[3];
+  uint64_t k_full[3], v_full[3];
+  uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
 };
 
 template <int D, bool BF16>
 __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_kernel(const __grid_constant__ FwdParams p) {
   using Cfg = FwdCfg<D>;
   constexpr int SW = Cfg::SW, BN = Cfg::BN, NST = Cfg::STAGES;
+  // d <= 64: P V of tile i and S of tile i + 1 form one MMA batch with one wait (both fit in 128 registers); larger d waits
+  // for each batch separately, since the O accumulator leaves no room for S next to the P fragments
+  constexpr bool kMerge = D <= 64;
   const int b = blockIdx.z, h = blockIdx.y;
   const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
   const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
@@ -97,27 +104,26 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
     for (int i = 0; i < NST; ++i) {
       mbar_init(&bars->k_full[i], 1);
       mbar_init(&bars->v_full[i], 1);
-      mbar_init(&bars->k_empty[i], 256);
-      mbar_init(&bars->v_empty[i], 256);
+      bars->k_free[i] = bars->v_free[i] = 0u;
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  // TMA issue (thread 0): Q and the first STAGES key tiles now; stage st is refilled once both warpgroups have released it
-  auto load_kv = [&](int i) {
+  // TMA issue of key tile i into its K or V stage (tm = &p.tmK / &p.tmV, off = Cfg::OFF_K / OFF_V, full = its full barriers)
+  auto load = [&](const CUtensorMap* tm, int off, uint64_t* full, int i) {
     const int st = i % NST;
-    const int kv_row = (int)(row0 + (long long)(t0 + i) * BN);
-    if (i >= NST) mbar_wait(&bars->k_empty[st], ((i / NST) - 1) & 1);
-    mbar_arrive_expect_tx(&bars->k_full[st], Cfg::KV_BYTES);
+    mbar_arrive_expect_tx(&full[st], Cfg::KV_BYTES);
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx)
-      tma_load_3d(smem + Cfg::OFF_K + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmK, &bars->k_full[st], bx * Cfg::BOX_COLS, h, kv_row);
-    if (i >= NST) mbar_wait(&bars->v_empty[st], ((i / NST) - 1) & 1);
-    mbar_arrive_expect_tx(&bars->v_full[st], Cfg::KV_BYTES);
-#pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX; ++bx)
-      tma_load_3d(smem + Cfg::OFF_V + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, &p.tmV, &bars->v_full[st], bx * Cfg::BOX_COLS, h, kv_row);
+      tma_load_3d(smem + off + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, tm, &full[st], bx * Cfg::BOX_COLS, h,
+                  (int)(row0 + (long long)(t0 + i) * BN));
+  };
+  // Thread 0 loads Q and the first STAGES key tiles.  Afterwards nobody waits for a free stage: each warp releases the K (V)
+  // stage of tile i once its MMAs that read it have completed, and the warp whose release is the last of the eight issues
+  // the load of tile i + STAGES into it, so neither warpgroup holds the other back.
+  auto release = [&](const CUtensorMap* tm, int off, uint64_t* full, uint32_t* ctr, int i) {
+    if (lane == 0 && i + NST < T && release_is_last<kFwdThreads / 32>(&ctr[i % NST])) load(tm, off, full, i + NST);
   };
   if (tid == 0) {
     prefetch_tensormap(&p.tmQ);
@@ -127,7 +133,10 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx)
       tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
-    for (int i = 0; i < min(T, NST); ++i) load_kv(i);
+    for (int i = 0; i < min(T, NST); ++i) {
+      load(&p.tmK, Cfg::OFF_K, bars->k_full, i);
+      load(&p.tmV, Cfg::OFF_V, bars->v_full, i);
+    }
   }
   __syncwarp();
 
@@ -146,24 +155,30 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
   for (int kk = 0; kk < BN / 16; ++kk)
 #pragma unroll
     for (int r = 0; r < 4; ++r) a_hi[kk][r] = a_lo[kk][r] = 0u;
-  mbar_wait(&bars->q_full, 0);
-  for (int i = 0; i < T; ++i) {
-    const int st = i % NST;
-    const uint32_t ph = (i / NST) & 1;
-    mbar_wait(&bars->k_full[st], ph);
-    float s[BN / 2];
-    wgmma_fence();
+  float s[BN / 2];
+  // S = Q K_i^T into s (issue only; the caller fences, commits and waits)
+  auto issue_s = [&](int i) {
+    const uint32_t kst = sk + (i % NST) * Cfg::KV_BYTES;
 #pragma unroll
     for (int ks = 0; ks < D / 16; ++ks) {
       const int kb = ks * 32, bx = kb / SW, off = kb % SW;
-      wgmma_ss<BN, BF16, 0, 0>(s, desc_kmajor<SW>(sq + bx * Cfg::Q_BOX, off),
-                               desc_kmajor<SW>(sk + st * Cfg::KV_BYTES + bx * Cfg::KV_BOX, off), ks > 0);
+      wgmma_ss<BN, BF16, 0, 0>(s, desc_kmajor<SW>(sq + bx * Cfg::Q_BOX, off), desc_kmajor<SW>(kst + bx * Cfg::KV_BOX, off), ks > 0);
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(s);
-    mbar_arrive(&bars->k_empty[st]);
-
+  };
+  mbar_wait(&bars->q_full, 0);
+  mbar_wait(&bars->k_full[0], 0);
+  wgmma_fence();
+  issue_s(0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(s);
+  release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, 0);
+  __syncwarp();
+  // Per tile i (s holds S_i): P_i -> A fragments; one MMA batch of O += P_i V_i and (kMerge) S_{i+1} = Q K_{i+1}^T; one wait;
+  // V_i and K_{i+1} are released.  O is never read inside the loop, so no MMA waits on the elementwise code of its own tile.
+  for (int i = 0; i < T; ++i) {
+    const int st = i % NST;
+    const bool next = i + 1 < T;
     const int n0 = (t0 + i) * BN;
     const bool full = n0 + BN <= full_lim;  // tile-uniform
 #pragma unroll
@@ -185,7 +200,8 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
       a_hi[kk][0] = x0.hi; a_hi[kk][1] = x1.hi; a_hi[kk][2] = x2.hi; a_hi[kk][3] = x3.hi;
       a_lo[kk][0] = x0.lo; a_lo[kk][1] = x1.lo; a_lo[kk][2] = x2.lo; a_lo[kk][3] = x3.lo;
     }
-    mbar_wait(&bars->v_full[st], ph);
+    mbar_wait(&bars->v_full[st], (i / NST) & 1);
+    if (kMerge && next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk) {
@@ -193,13 +209,23 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
       wgmma_rs<D, BF16, 1>(o, a_hi[kk], vd, 1);
       if constexpr (BF16) wgmma_rs<D, BF16, 1>(o, a_lo[kk], vd, 1);
     }
+    if (kMerge && next) issue_s(i + 1);
     wgmma_commit();
     wgmma_wait<0>();  // an MMA batch never stays in flight across the elementwise code (ptxas would serialise them)
     fence_regs(o);
     fence_regs(a_hi);
     fence_regs(a_lo);
-    mbar_arrive(&bars->v_empty[st]);
-    if (tid == 0 && i + NST < T) load_kv(i + NST);  // K and V of tile i are no longer read
+    fence_regs(s);
+    release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i);
+    if (!kMerge && next) {
+      mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+      wgmma_fence();
+      issue_s(i + 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+    }
+    if (next) release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i + 1);
     __syncwarp();
   }
 

@@ -68,6 +68,17 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 #endif
 
+// Release of a TMA ring stage without a waiting producer: every warp calls this once per use of the stage (lane 0, after the
+// wgmma wait that ends the warp's reads of it), and the call that completes the release -- the COUNT-th of that use -- returns
+// true; that warp issues the refill.  COUNT is a power of two; `ctr` starts at 0 and only grows.
+template <uint32_t COUNT>
+__device__ __forceinline__ bool release_is_last(uint32_t* ctr) {
+  static_assert((COUNT & (COUNT - 1)) == 0, "COUNT must be a power of two");
+  uint32_t old;
+  asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"(smem_u32(ctr)) : "memory");
+  return ((old + 1) & (COUNT - 1)) == 0;
+}
+
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -160,16 +171,18 @@ __device__ __forceinline__ float tanh_approx(float x) {
 }
 
 // A 16-bit MMA operand computed in fp32 (P or dS).  wgmma takes ONE format for A and B, so with bf16 inputs the operand is
-// bf16, and its 8-bit significand alone costs ~1.7e-3 of relative error.  It is therefore split into hi = bf16(x) and
-// lo = bf16(x - hi) (16 significant bits together) and multiplied twice; fp16 inputs use one fp16 operand (11 bits).
+// bf16, and its 8-bit significand alone costs ~1.7e-3 of relative error.  It is therefore split into hi = x truncated to
+// bf16 (its upper 16 bits, one byte permute for the pair) and lo = bf16_rn(x - hi), and multiplied twice.  x - hi is exact
+// in fp32 and below 2^-7 |x|, so the pair is within 2^-16 |x| of x at the cost of one conversion per pair of values; fp16
+// inputs use one fp16 operand (11 bits).
 template <bool BF16>
 struct Operand {
   uint32_t hi, lo;
   __device__ __forceinline__ Operand(float a, float b) {
     if constexpr (BF16) {
-      hi = pack_bf16x2(a, b);
-      const float ha = __uint_as_float(hi << 16), hb = __uint_as_float(hi & 0xffff0000u);
-      lo = pack_bf16x2(a - ha, b - hb);
+      const uint32_t ua = __float_as_uint(a), ub = __float_as_uint(b);
+      asm("prmt.b32 %0, %1, %2, 0x7632;" : "=r"(hi) : "r"(ua), "r"(ub));
+      lo = pack_bf16x2(a - __uint_as_float(ua & 0xffff0000u), b - __uint_as_float(ub & 0xffff0000u));
     } else {
       hi = pack_f16x2_sat(a, b);
       lo = 0u;

@@ -6,7 +6,8 @@ for phase k while phase k-1 has not completed sees the parity test succeed at on
 (4) no TMA load is issued into a Q / dO stage that a warpgroup still reads, and (5) no dS buffer is written while the dQ
 MMA of an earlier tile reads it, or read while it is written.
 
-Actors: the two warpgroups W0 / W1 (128 threads each, modelled as one arrival each); thread 0 of W0 also issues the TMA loads.
+Actors: the eight warps W0..W7 of the two warpgroups (W0-W3 and W4-W7).  Thread 0 (in W0) issues the first TMA loads; after
+that a stage is refilled by the warp whose release completes it (Release, below), so nobody waits for a free stage.
 TMA completions are asynchronous: queued per issuing actor and fired later, in order.
 usage: sim_bwd_protocol.py [--d 32|64|128] [--tiles T] [--seeds N] [--break-ds]"""
 import argparse
@@ -27,6 +28,30 @@ class Bar:
 
 class Violation(Exception):
     pass
+
+
+WARPS = 8  # one release per warp and use of a stage (release_is_last<8> in csrc/wgmma.cuh)
+
+
+class Release:
+    """Release counter of one ring stage: WARPS arrivals per use, and arrival number `refill_at` of a use (the last one in the
+    kernels) is told to refill the stage.  A smaller `refill_at` seeds a break."""
+
+    def __init__(self, refill_at=WARPS):
+        self.refill_at, self.n = refill_at, 0
+
+    def arrive(self):
+        self.n += 1
+        return (self.n - 1) % WARPS + 1 == self.refill_at
+
+
+def release(ctr, refill):
+    """One warp's release of a stage (an atomic step); if it is the refilling arrival, the warp then issues `refill` (a list of
+    ops, usually TMA loads)."""
+    got = []
+    yield ("call", lambda: got.append(ctr.arrive()))
+    if got[0]:
+        yield from refill
 
 
 def _simulate(actors, B, rnd):
@@ -67,6 +92,8 @@ def _simulate(actors, B, rnd):
                     continue
             elif op[0] == "arrive":
                 B[op[1]].arrive()
+            elif op[0] == "call":        # an atomic step of the actor's own (a shared-memory atomic)
+                op[1]()
             elif op[0] == "async":
                 queues[k].append(op[1])
             elif op[0] == "tma":          # TMA load into stage op[2], completing on barrier op[1]
@@ -97,10 +124,11 @@ def run(T, d, seed, break_ds=False):
     NST = STAGES[d]
     NDS = 1 if break_ds else 2
     rnd = random.Random(seed)
-    B = {"kv": Bar(1), "nb": Bar(2)}
+    B = {"kv": Bar(1), "nb": Bar(WARPS)}
+    R = {}
     for i in range(NST):
-        B[f"qf{i}"] = Bar(1)   # expect_tx arrival of thread 0 + TMA bytes: modelled as the TMA completion
-        B[f"qe{i}"] = Bar(2)   # 256 consumer threads: one arrival per warpgroup
+        B[f"qf{i}"] = Bar(1)   # expect_tx arrival of the loading thread + TMA bytes: modelled as the TMA completion
+        R[i] = Release()
 
     def W(w):
         if w == 0:                                   # thread 0: K / V and the first STAGES query tiles
@@ -113,35 +141,37 @@ def run(T, d, seed, break_ds=False):
             yield ("wait", f"qf{st}", j // NST)
             yield ("read", f"q{st}", 1)              # S^T, dP^T, dV, dK MMAs read Q_j / dO_j ...
             yield ("read", f"q{st}", -1)             # ... and complete within the iteration
-            yield ("arrive", f"qe{st}")
-            if w == 0 and j + NST < T:               # refill the stage once both warpgroups have released it
-                yield ("wait", f"qe{st}", j // NST)
-                yield ("tma", f"qf{st}", f"q{st}")
+            if j + NST < T:                          # the last warp to release the stage refills it
+                yield from release(R[st], [("tma", f"qf{st}", f"q{st}")])
             b = f"ds{j % NDS}"
-            yield ("write", b, 1)                    # dS^T of this warpgroup's 64 keys
+            yield ("write", b, 1)                    # dS^T of this warp's 16 keys
             yield ("write", b, -1)
             yield ("arrive", "nb")                   # named barrier of the 256 consumer threads
             yield ("wait", "nb", j)
-            if j % 2 == w:                           # dQ_j = dS K, waited for before the warpgroup goes on
+            if j % 2 == w // 4:                      # dQ_j = dS K by warpgroup j % 2, waited for before the warp goes on
                 yield ("read", b, 1)
                 yield ("read", b, -1)
 
-    return _simulate({"W0": W(0), "W1": W(1)}, B, rnd)
+    return _simulate({f"W{w}": W(w) for w in range(WARPS)}, B, rnd)
 
 
 DKDV_STAGES = 4  # BwdCfg<32, false>::STAGES
 
 
-def run_dkdv(T, seed, break_release=False):
-    """attn_bwd_dkdv_wgmma_kernel (d = 32): the key-tile CTA of `run` without dS buffers, named barrier or dQ; the two
-    warpgroups meet only at the Q / dO empty barriers.  break_release: thread 0 refills a stage once its own warpgroup has
-    released it, without waiting for the other one (must be caught)."""
+def run_dkdv(T, seed, break_release=False, first_releaser=False, early_release=False):
+    """attn_bwd_dkdv_wgmma_kernel (d = 32): the key-tile CTA of `run` without dS buffers, named barrier or dQ; the warps meet
+    only at the Q / dO ring.  Seeded breaks (each must be caught):
+      break_release   the stage is refilled once four warps (one warpgroup's worth) have released it;
+      first_releaser  the first warp to release the stage refills it;
+      early_release   a warp releases Q_j / dO_j before the wait of the MMAs that read them."""
     NST = DKDV_STAGES
+    refill_at = 1 if first_releaser else WARPS // 2 if break_release else WARPS
     rnd = random.Random(seed)
     B = {"kv": Bar(1)}
+    R = {}
     for i in range(NST):
         B[f"qf{i}"] = Bar(1)
-        B[f"qe{i}"] = Bar(2)
+        R[i] = Release(refill_at)
 
     def W(w):
         if w == 0:
@@ -151,16 +181,16 @@ def run_dkdv(T, seed, break_release=False):
         yield ("wait", "kv", 0)
         for j in range(T):
             st = j % NST
+            refill = [("tma", f"qf{st}", f"q{st}")]
             yield ("wait", f"qf{st}", j // NST)
-            yield ("read", f"q{st}", 1)              # S^T, dP^T, dV, dK MMAs, waited for
-            yield ("read", f"q{st}", -1)
-            yield ("arrive", f"qe{st}")
-            if w == 0 and j + NST < T:
-                if not break_release:
-                    yield ("wait", f"qe{st}", j // NST)
-                yield ("tma", f"qf{st}", f"q{st}")
+            yield ("read", f"q{st}", 1)              # S^T, dP^T, dV, dK MMAs ...
+            if early_release and j + NST < T:
+                yield from release(R[st], refill)
+            yield ("read", f"q{st}", -1)             # ... waited for
+            if not early_release and j + NST < T:
+                yield from release(R[st], refill)
 
-    return _simulate({"W0": W(0), "W1": W(1)}, B, rnd)
+    return _simulate({f"W{w}": W(w) for w in range(WARPS)}, B, rnd)
 
 
 def main():
