@@ -22,8 +22,8 @@
 // Operand), so that their rounding stays inside the 1e-3 parity budget whatever the scale of dO.
 //
 //
-// d = 32 runs two kernels instead, with no atomics and no coupling between the warpgroups (DESIGN.md 3.2):
-//   attn_bwd_dkdv_wgmma_kernel  the kernel above without the dS buffers, the named barrier and dQ: dK and dV only.
+// d = 32 runs two kernels instead, with no atomics and no per-tile coupling between the warpgroups (DESIGN.md 3.2):
+//   attn_bwd_dkdv_wgmma_kernel  the kernel above without the dS buffers, the dS barrier and dQ: dK and dV only.
 //   attn_bwd_dq_wgmma_kernel    query-stationary, shaped like the forward: one CTA per (128-row query tile, head, sequence),
 //                               Q and dO resident, K and V streamed in 64-key tiles; it recomputes S = Q K^T and
 //                               dP = dO V^T, forms dS from one tanh and accumulates dQ += dS K in registers.  Its K / V ring
@@ -100,7 +100,8 @@ struct QTiles {
 };
 
 // Body of the key-stationary kernels: FUSED_DQ = attn_bwd_wgmma_kernel (dK, dV and the dQ atomics), otherwise
-// attn_bwd_dkdv_wgmma_kernel (dK and dV only; the warpgroups meet only at the ring's empty barriers).
+// attn_bwd_dkdv_wgmma_kernel (dK and dV only; the warpgroups meet at the ring and once at the query tile that crosses the
+// sequence end).
 template <int D, bool BF16, bool FUSED_DQ>
 __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   using Cfg = BwdCfg<D, FUSED_DQ>;
@@ -190,11 +191,26 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     for (int r = 0; r < 4; ++r) pf_hi[kk][r] = pf_lo[kk][r] = df_hi[kk][r] = df_lo[kk][r] = 0u;
 
   mbar_wait(&bars->kv_full, 0);
+  // K rows >= len of a key tile that crosses the sequence end are B of dQ = dS K (dS is 0 there, K may be NaN)
+  if (FUSED_DQ && n0 + Cfg::BKV > len) {  // CTA-uniform; K is loaded once
+    zero_tile_rows<Cfg::BKV, SW, Cfg::NBOX, kBwdThreads>(smem + Cfg::OFF_K, len - n0);
+    fence_proxy_async_smem();
+    named_bar_sync(kBarZeroRows, kBwdThreads);
+  }
   for (int j = 0; j < qt.T; ++j) {
     const int st = j % NST;
     const uint32_t ph = (j / NST) & 1;
     const int q0 = qt.at(j) * BQ;
     mbar_wait(&bars->qd_full[st], ph);
+    // Q_j / dO_j rows >= len are B of dK += dS^T Q_j and dV += P^T dO_j (P and dS are 0 there, Q / dO may be NaN).  The query
+    // tile that crosses the sequence end is the last one of the key tile (hi <= len, ctx_hi <= len), so its stage is not
+    // refilled after the zeroing.
+    if (q0 + BQ > len) {  // CTA-uniform
+      zero_tile_rows<BQ, SW, Cfg::NBOX, kBwdThreads>(smem + Cfg::OFF_Q + st * Cfg::QD_BYTES, len - q0);
+      zero_tile_rows<BQ, SW, Cfg::NBOX, kBwdThreads>(smem + Cfg::OFF_DO + st * Cfg::QD_BYTES, len - q0);
+      fence_proxy_async_smem();
+      named_bar_sync(kBarZeroRows, kBwdThreads);
+    }
     float s[32], dp[32];
     wgmma_fence();
 #pragma unroll
@@ -495,9 +511,16 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
     const int st = i % NST;
     const uint32_t ph = (i / NST) & 1;
     const uint32_t kst = sk + st * Cfg::KV_BYTES, vst = sv + st * Cfg::KV_BYTES;
+    const int n0 = (t0 + i) * BN;
     float s[BN / 2], dp[BN / 2];
     mbar_wait(&bars->k_full[st], ph);
     mbar_wait(&bars->v_full[st], ph);
+    // the last key tile may cross the sequence end: its K rows >= len are B of dQ += dS K (dS is 0 there, K may be NaN)
+    if (n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
+      zero_tile_rows<BN, SW, Cfg::NBOX, kBwdThreads>(smem + Cfg::OFF_K + st * Cfg::KV_BYTES, len - n0);
+      fence_proxy_async_smem();
+      named_bar_sync(kBarZeroRows, kBwdThreads);
+    }
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < D / 16; ++ks) {
@@ -517,7 +540,6 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
     __syncwarp();
 
     // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2
-    const int n0 = (t0 + i) * BN;
     const bool full = n0 + BN <= full_lim;  // tile-uniform
 #pragma unroll
     for (int nb = 0; nb < BN / 8; ++nb)

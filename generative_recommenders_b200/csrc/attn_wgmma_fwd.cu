@@ -17,7 +17,8 @@
 // P is a 16-bit MMA operand of the same format as V (wgmma takes one format for A and B): fp16 for fp16 inputs, and for
 // bf16 inputs a hi + lo pair of bf16 operands multiplied twice (wgmma.cuh, Operand), so that its rounding stays well inside
 // the 1e-3 parity budget.  The 1/N factor of the reference is applied once in the epilogue (registers -> global, rows past
-// the sequence end are not written).  Rows of neighbouring sequences that a TMA box drags in are neutralised by the mask.
+// the sequence end are not written).  Rows past the sequence end that a TMA box drags in are masked out of P, and zeroed in the
+// V stage of the one key tile that crosses the end (zero_tile_rows), since P = 0 does not neutralise a NaN or Inf in V.
 //
 // Reference semantics: ops/pytorch/pt_hstu_attention.py:130-171; tile skipping mirrors the idea of
 // ops/triton/triton_hstu_attention.py:517-543 (loop bounds from the mask) but is derived from common.cuh's ranges.
@@ -201,6 +202,12 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
       a_lo[kk][0] = x0.lo; a_lo[kk][1] = x1.lo; a_lo[kk][2] = x2.lo; a_lo[kk][3] = x3.lo;
     }
     mbar_wait(&bars->v_full[st], (i / NST) & 1);
+    // the last tile may cross the sequence end: its V rows >= len belong to the next sequence (P is 0 there, V may be NaN)
+    if (n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
+      zero_tile_rows<BN, SW, Cfg::NBOX, kFwdThreads>(smem + Cfg::OFF_V + st * Cfg::KV_BYTES, len - n0);
+      fence_proxy_async_smem();
+      named_bar_sync(kBarZeroRows, kFwdThreads);
+    }
     if (kMerge && next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
     wgmma_fence();
 #pragma unroll

@@ -84,6 +84,25 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// Zeroes rows [r0, ROWS) of a TMA-loaded tile of NBOX swizzled boxes of [ROWS][SW bytes] (a row is one contiguous SW-byte line
+// of its box whatever the swizzle), so that rows a box dragged in past a sequence end cannot reach an MMA: a zero in the
+// other factor does not neutralise them, 0 * NaN = NaN.  Called by all NTHREADS threads of the CTA after the tile's full
+// barrier; the caller then issues fence_proxy_async_smem() and a CTA-wide named barrier, so that no warpgroup's wgmma reads
+// the tile before every row is zero, and makes sure the stage is not refilled while the zeros are still needed.
+template <int ROWS, int SW, int NBOX, int NTHREADS>
+__device__ __forceinline__ void zero_tile_rows(uint8_t* tile, int r0) {
+  constexpr int kChunks = ROWS * SW / 16;  // 16-byte chunks per box, a fixed number per thread (few registers)
+  static_assert(kChunks % NTHREADS == 0, "whole chunks per thread");
+#pragma unroll
+  for (int bx = 0; bx < NBOX; ++bx)
+#pragma unroll
+    for (int k = 0; k < kChunks / NTHREADS; ++k) {
+      const int c = k * NTHREADS + (int)threadIdx.x;
+      if (c >= r0 * (SW / 16)) *reinterpret_cast<uint4*>(tile + bx * ROWS * SW + c * 16) = make_uint4(0u, 0u, 0u, 0u);
+    }
+}
+constexpr int kBarZeroRows = 2;  // named barrier after zero_tile_rows (0 is __syncthreads, 1 the fused backward's dS barrier)
+
 // ---------------------------------------------------------------------------------------------
 // TMA loads (tile mode) into shared memory, completion on an mbarrier
 // ---------------------------------------------------------------------------------------------

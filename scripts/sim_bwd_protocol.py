@@ -45,6 +45,17 @@ class Release:
         return (self.n - 1) % WARPS + 1 == self.refill_at
 
 
+def zero_rows(res, barrier, phase, skip_barrier=False):
+    """All eight warps zero the rows past the sequence end of stage `res` (zero_tile_rows, csrc/wgmma.cuh: plain stores, then
+    fence.proxy.async), then meet at the CTA-wide named barrier `barrier` before any MMA reads the stage.  skip_barrier seeds
+    the break of reading the stage without the barrier."""
+    yield ("write", res, 1)
+    yield ("write", res, -1)
+    if not skip_barrier:
+        yield ("arrive", barrier)
+        yield ("wait", barrier, phase)
+
+
 def release(ctr, refill):
     """One warp's release of a stage (an atomic step); if it is the refilling arrival, the warp then issues `refill` (a list of
     ops, usually TMA loads)."""
@@ -99,6 +110,8 @@ def _simulate(actors, B, rnd):
             elif op[0] == "tma":          # TMA load into stage op[2], completing on barrier op[1]
                 if readers.get(op[2], 0):
                     raise Violation(f"{k}: TMA load into {op[2]} while it is being read")
+                if writers.get(op[2], 0):
+                    raise Violation(f"{k}: TMA load into {op[2]} while it is being written")
                 queues[k].append(op[1])
             elif op[0] in ("read", "write"):
                 _, res, delta = op
@@ -119,12 +132,14 @@ def _simulate(actors, B, rnd):
     return steps
 
 
-def run(T, d, seed, break_ds=False):
-    """One key-tile CTA streaming T query tiles.  break_ds: one dS buffer instead of two (must be caught)."""
+def run(T, d, seed, break_ds=False, straddle=True, break_zero=False):
+    """One key-tile CTA streaming T query tiles.  straddle: the key tile and the last query tile cross the sequence end, so K
+    and that Q_j / dO_j stage get their rows past it zeroed.  Seeded breaks (each must be caught): break_ds, one dS buffer
+    instead of two; break_zero, no named barrier between the zeroing and the MMAs."""
     NST = STAGES[d]
     NDS = 1 if break_ds else 2
     rnd = random.Random(seed)
-    B = {"kv": Bar(1), "nb": Bar(WARPS)}
+    B = {"kv": Bar(1), "nb": Bar(WARPS), "zb": Bar(WARPS)}
     R = {}
     for i in range(NST):
         B[f"qf{i}"] = Bar(1)   # expect_tx arrival of the loading thread + TMA bytes: modelled as the TMA completion
@@ -136,9 +151,13 @@ def run(T, d, seed, break_ds=False):
             for j in range(min(T, NST)):
                 yield ("tma", f"qf{j % NST}", f"q{j % NST}")
         yield ("wait", "kv", 0)
+        if straddle:
+            yield from zero_rows("k", "zb", 0, break_zero)
         for j in range(T):
             st = j % NST
             yield ("wait", f"qf{st}", j // NST)
+            if straddle and j == T - 1:
+                yield from zero_rows(f"q{st}", "zb", 1, break_zero)
             yield ("read", f"q{st}", 1)              # S^T, dP^T, dV, dK MMAs read Q_j / dO_j ...
             yield ("read", f"q{st}", -1)             # ... and complete within the iteration
             if j + NST < T:                          # the last warp to release the stage refills it
@@ -150,6 +169,8 @@ def run(T, d, seed, break_ds=False):
             yield ("wait", "nb", j)
             if j % 2 == w // 4:                      # dQ_j = dS K by warpgroup j % 2, waited for before the warp goes on
                 yield ("read", b, 1)
+                yield ("read", "k", 1)
+                yield ("read", "k", -1)
                 yield ("read", b, -1)
 
     return _simulate({f"W{w}": W(w) for w in range(WARPS)}, B, rnd)
@@ -158,16 +179,18 @@ def run(T, d, seed, break_ds=False):
 DKDV_STAGES = 4  # BwdCfg<32, false>::STAGES
 
 
-def run_dkdv(T, seed, break_release=False, first_releaser=False, early_release=False):
-    """attn_bwd_dkdv_wgmma_kernel (d = 32): the key-tile CTA of `run` without dS buffers, named barrier or dQ; the warps meet
-    only at the Q / dO ring.  Seeded breaks (each must be caught):
+def run_dkdv(T, seed, break_release=False, first_releaser=False, early_release=False, straddle=True, break_zero=False):
+    """attn_bwd_dkdv_wgmma_kernel (d = 32): the key-tile CTA of `run` without dS buffers, dS barrier or dQ; the warps meet at
+    the Q / dO ring and, with `straddle`, once at the named barrier after zeroing the rows of the last query tile that lie
+    past the sequence end.  Seeded breaks (each must be caught):
+      break_zero      no named barrier between that zeroing and the MMAs;
       break_release   the stage is refilled once four warps (one warpgroup's worth) have released it;
       first_releaser  the first warp to release the stage refills it;
       early_release   a warp releases Q_j / dO_j before the wait of the MMAs that read them."""
     NST = DKDV_STAGES
     refill_at = 1 if first_releaser else WARPS // 2 if break_release else WARPS
     rnd = random.Random(seed)
-    B = {"kv": Bar(1)}
+    B = {"kv": Bar(1), "zb": Bar(WARPS)}
     R = {}
     for i in range(NST):
         B[f"qf{i}"] = Bar(1)
@@ -183,6 +206,8 @@ def run_dkdv(T, seed, break_release=False, first_releaser=False, early_release=F
             st = j % NST
             refill = [("tma", f"qf{st}", f"q{st}")]
             yield ("wait", f"qf{st}", j // NST)
+            if straddle and j == T - 1:
+                yield from zero_rows(f"q{st}", "zb", 0, break_zero)
             yield ("read", f"q{st}", 1)              # S^T, dP^T, dV, dK MMAs ...
             if early_release and j + NST < T:
                 yield from release(R[st], refill)

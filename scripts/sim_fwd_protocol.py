@@ -17,20 +17,23 @@ _spec = importlib.util.spec_from_file_location("sim_bwd_protocol", os.path.join(
                                                                                  "sim_bwd_protocol.py"))
 _eng = importlib.util.module_from_spec(_spec)
 _spec.loader.exec_module(_eng)
-Bar, Violation, Release, WARPS, release = _eng.Bar, _eng.Violation, _eng.Release, _eng.WARPS, _eng.release
+Bar, Violation, Release, WARPS, release, zero_rows = (_eng.Bar, _eng.Violation, _eng.Release, _eng.WARPS, _eng.release,
+                                                      _eng.zero_rows)
 
 STAGES = {32: 3, 64: 3, 128: 3, 256: 2}  # FwdCfg<D>::STAGES
 
 
-def run(T, d, seed, break_refill=False, first_releaser=False, early_release=False):
-    """One query-tile CTA over T key tiles.  Seeded breaks (each must be caught):
+def run(T, d, seed, break_refill=False, first_releaser=False, early_release=False, straddle=True, break_zero=False):
+    """One query-tile CTA over T key tiles; with `straddle` the last key tile crosses the sequence end, and all warps zero
+    its V rows past the end and meet at a named barrier before O += P V reads them.  Seeded breaks (each must be caught):
+      break_zero                    no named barrier between that zeroing and the MMAs;
       break_refill, first_releaser  the first warp to release a stage refills it;
       early_release                 (d <= 64) K_{i+1} is released before the wait of the batch that reads it."""
     NST = STAGES[d]
     merge = d <= 64
     refill_at = 1 if (break_refill or first_releaser) else WARPS
     rnd = random.Random(seed)
-    B = {"q": Bar(1)}
+    B = {"q": Bar(1), "zb": Bar(WARPS)}
     R = {}
     for i in range(NST):
         B[f"kf{i}"], B[f"vf{i}"] = Bar(1), Bar(1)
@@ -56,6 +59,8 @@ def run(T, d, seed, break_refill=False, first_releaser=False, early_release=Fals
             st, nst = i % NST, (i + 1) % NST
             nxt = i + 1 < T
             yield ("wait", f"vf{st}", i // NST)
+            if straddle and not nxt:
+                yield from zero_rows(f"v{st}", "zb", 0, break_zero)
             if merge and nxt:
                 yield ("wait", f"kf{nst}", (i + 1) // NST)
             yield ("read", f"v{st}", 1)              # O += P_i V_i ...
@@ -80,9 +85,12 @@ def run(T, d, seed, break_refill=False, first_releaser=False, early_release=Fals
 DQ_STAGES = 3  # DqCfg<32>::STAGES (csrc/attn_wgmma_bwd.cu)
 
 
-def run_dq(T, seed, break_k_refill=False, first_releaser=False, early_release=False):
+def run_dq(T, seed, break_k_refill=False, first_releaser=False, early_release=False, straddle=True, break_zero=False):
     """attn_bwd_dq_wgmma_kernel (d = 32): the forward's ring with Q and dO resident; S / dP read K and V and are waited for,
-    V is released, then dQ += dS K reads K, is waited for, and K is released.  Seeded breaks (each must be caught):
+    V is released, then dQ += dS K reads K, is waited for, and K is released.  With `straddle` the last key tile crosses the
+    sequence end, and all warps zero its K rows past the end and meet at a named barrier first.  Seeded breaks (each must be
+    caught):
+      break_zero      no named barrier between that zeroing and the MMAs;
       break_k_refill  the K stage is refilled by the warp that completes the release of V (after S / dP) instead of K, so
                       the load may land while another warp's dQ MMA still reads K;
       first_releaser  the first warp to release a stage refills it;
@@ -90,7 +98,7 @@ def run_dq(T, seed, break_k_refill=False, first_releaser=False, early_release=Fa
     NST = DQ_STAGES
     refill_at = 1 if first_releaser else WARPS
     rnd = random.Random(seed)
-    B = {"qd": Bar(1)}
+    B = {"qd": Bar(1), "zb": Bar(WARPS)}
     R = {}
     for i in range(NST):
         B[f"kf{i}"], B[f"vf{i}"] = Bar(1), Bar(1)
@@ -108,6 +116,8 @@ def run_dq(T, seed, break_k_refill=False, first_releaser=False, early_release=Fa
             k_load, v_load = [("tma", f"kf{st}", f"k{st}")], [("tma", f"vf{st}", f"v{st}")]
             yield ("wait", f"kf{st}", i // NST)
             yield ("wait", f"vf{st}", i // NST)
+            if straddle and i == T - 1:
+                yield from zero_rows(f"k{st}", "zb", 0, break_zero)
             yield ("read", f"k{st}", 1)          # S = Q K^T and dP = dO V^T, waited for
             yield ("read", f"v{st}", 1)
             yield ("read", f"v{st}", -1)

@@ -118,13 +118,15 @@ def test_attention_random_grid_generic(idx):
 
 @pytest.mark.parametrize("d", [32, 64, 128])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("opts", [(False, False, 0, 0), (True, False, 0, 0), (True, True, 0, 0), (True, True, 7, 0),
-                                  (True, True, 5, 33), (False, False, 4, 0)])
+@pytest.mark.parametrize("opts", [(False, False, 0, 0, False), (True, False, 0, 0, False), (True, True, 0, 0, False),
+                                  (True, True, 7, 0, False), (True, True, 5, 33, False), (False, False, 4, 0, False),
+                                  (True, False, 0, 0, True), (True, True, 5, 33, True)])
 def test_attention_umma_vs_oracle(d, dtype, opts):
-    """wgmma/TMA forward (+ backward of whichever implementation AUTO selects) against the fp32 oracle."""
+    """wgmma/TMA forward (+ backward of whichever implementation AUTO selects) against the fp32 oracle; the last element of
+    `opts` passes seq_offsets / num_targets as int32 instead of int64."""
     _lib = _mods()[0]
-    targets, window, ctx, min_full = opts
-    case = _random_case(7000 + d + ctx, dtype, 5, 3, 300, 24, d, d, targets, window, ctx, min_full)
+    targets, window, ctx, min_full, i32 = opts
+    case = _random_case(7000 + d + ctx, dtype, 5, 3, 300, 24, d, d, targets, window, ctx, min_full, i32=i32)
     assert _selected(case, _lib) == _lib.IMPL_UMMA
     _check_vs_oracle(case, _lib.IMPL_UMMA, f"umma-d{d}-{dtype}-{opts}")
 

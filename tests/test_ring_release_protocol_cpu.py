@@ -56,3 +56,25 @@ def test_unmerged_forward_catches_a_refill_by_the_first_releaser(d):
     with pytest.raises(Violation, match="TMA load into|wait on"):
         for seed in range(100):
             fwd.run(8, d, seed, first_releaser=True)
+
+
+ZERO_MODELS = dict(MODELS, fused64=lambda T, s, **kw: bwd.run(T, 64, s, **kw),
+                   fused128=lambda T, s, **kw: bwd.run(T, 128, s, **kw))
+
+
+@pytest.mark.parametrize("model", sorted(ZERO_MODELS))
+def test_zeroing_rows_past_the_sequence_end_holds_under_many_schedules(model):
+    """All warps zero the rows past the sequence end of the tile that crosses it (the last key tile of the forward and the dQ
+    kernel; the key tile and the last query tile of the key-stationary kernels), then meet at one named barrier."""
+    for straddle in (False, True):
+        for tiles in (1, 2, 3, 4, 5, 9):
+            for seed in range(60):
+                ZERO_MODELS[model](tiles, 2000 + seed, straddle=straddle)
+
+
+@pytest.mark.parametrize("model", sorted(ZERO_MODELS))
+def test_model_catches_zeroing_without_the_barrier(model):
+    with pytest.raises(Violation, match="while it is being (written|read)"):
+        for seed in range(200):
+            for tiles in (1, 3):
+                ZERO_MODELS[model](tiles, seed, break_zero=True)
