@@ -1,0 +1,152 @@
+// Pre-pass of the bf16 d = 32 wgmma attention: per (sequence, head) amax of the operands and their exactly scaled fp16
+// copies (attn_fp16_operands.cuh, DESIGN.md 3.0).  Two kernels on the caller's stream, before the attention kernels:
+//   fp16_operands_amax_kernel     atomicMax of the bits of |x| (order-independent, so the result is bitwise reproducible)
+//   fp16_operands_convert_kernel  x * 2^e as fp16 into the workspace, [L, H, 32] per operand
+// Both run one CTA per (256-row block, head, sequence) over the rows < max_seq_len of each sequence.  Rows of the copies
+// past max_seq_len are not written: the attention kernels treat them as rows past the sequence end, which never reach an
+// MMA (zero_tile_rows, DESIGN.md 2).
+#include <cuda_fp16.h>
+#include <string.h>
+
+#include "attn_fp16_operands.cuh"
+#include "common.cuh"
+#include "internal.h"
+
+namespace hstu {
+
+constexpr int kPreRows = 256, kPreThreads = 256, kPreD = 32;
+
+struct PreOperand {
+  const uint16_t* src;  // bf16 [L, H, 32] view
+  long long row_stride, head_stride;
+  __half* dst;          // fp16 [L, H, 32], contiguous
+};
+
+struct PreParams {
+  PreOperand op[kAmaxSlots];
+  int nops;  // 3 (q, k, v) or 4 (+ dO)
+  const void* seq_offsets;
+  int offsets_i64, max_seq_len, heads;
+  float alpha;
+  uint32_t* amax;  // [B, H, kAmaxSlots], zeroed before the amax kernel
+};
+
+__device__ __forceinline__ float bf16_bits_to_float(uint32_t b) { return __uint_as_float(b << 16); }
+
+__global__ void __launch_bounds__(kPreThreads) fp16_operands_amax_kernel(const __grid_constant__ PreParams p) {
+  const int b = blockIdx.z, h = blockIdx.y;
+  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
+  const int len = min((int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0), p.max_seq_len);
+  const int r0 = blockIdx.x * kPreRows;
+  if (r0 >= len) return;
+  const int rows = min(kPreRows, len - r0);
+  __shared__ uint32_t red[kAmaxSlots][kPreThreads / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int o = 0; o < p.nops; ++o) {
+    const PreOperand& op = p.op[o];
+    uint32_t m = 0u;
+    // 4 threads per row, 8 elements (16 bytes) each
+    for (int c = threadIdx.x; c < rows * 4; c += kPreThreads) {
+      const int r = c >> 2, part = c & 3;
+      const uint4 x = *reinterpret_cast<const uint4*>(op.src + (row0 + r0 + r) * op.row_stride + (long long)h * op.head_stride + part * 8);
+      const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        // |x| as fp32 bits: the bf16 bits without the sign, shifted up (NaN sorts above Inf, Inf above every finite value)
+        m = max(m, (w[i] & 0x7fffu) << 16);
+        m = max(m, (w[i] >> 16 & 0x7fffu) << 16);
+      }
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, s));
+    if (lane == 0) red[o][warp] = m;
+  }
+  __syncthreads();
+  if (threadIdx.x < p.nops) {
+    uint32_t m = 0u;
+#pragma unroll
+    for (int w = 0; w < kPreThreads / 32; ++w) m = max(m, red[threadIdx.x][w]);
+    if (m) atomicMax(p.amax + ((long long)b * p.heads + h) * kAmaxSlots + threadIdx.x, m);
+  }
+}
+
+__global__ void __launch_bounds__(kPreThreads) fp16_operands_convert_kernel(const __grid_constant__ PreParams p) {
+  const int b = blockIdx.z, h = blockIdx.y;
+  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
+  const int len = min((int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0), p.max_seq_len);
+  const int r0 = blockIdx.x * kPreRows;
+  if (r0 >= len) return;
+  const int rows = min(kPreRows, len - r0);
+  const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, p.alpha, kPreD);
+  const int exps[kAmaxSlots] = {ex.q, ex.k, ex.v, ex.o};
+  for (int o = 0; o < p.nops; ++o) {
+    const PreOperand& op = p.op[o];
+    const int e = exps[o];
+    for (int c = threadIdx.x; c < rows * 4; c += kPreThreads) {
+      const int r = c >> 2, part = c & 3;
+      const long long row = row0 + r0 + r;
+      const uint4 x = *reinterpret_cast<const uint4*>(op.src + row * op.row_stride + (long long)h * op.head_stride + part * 8);
+      const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+      uint32_t y[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        // exact: a power-of-two scale of an 8-bit significand into fp16's range (scalbnf is exact wherever the result is)
+        const __half2 v = __floats2half2_rn(scalbnf(bf16_bits_to_float(w[i] & 0xffffu), e), scalbnf(bf16_bits_to_float(w[i] >> 16), e));
+        y[i] = *reinterpret_cast<const uint32_t*>(&v);
+      }
+      *reinterpret_cast<uint4*>(op.dst + (row * p.heads + h) * kPreD + part * 8) = make_uint4(y[0], y[1], y[2], y[3]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// host
+// ------------------------------------------------------------------------------------------------
+static size_t align256(size_t n) { return (n + 255) / 256 * 256; }
+
+size_t fp16_operands_workspace_bytes(const hstu_attn_params& p, bool bwd) {
+  const size_t amax = align256((size_t)p.batch * p.heads * kAmaxSlots * sizeof(uint32_t));
+  const size_t copy = align256((size_t)p.total_rows * p.heads * kPreD * sizeof(__half));
+  return amax + (bwd ? 4 : 3) * copy;
+}
+
+int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out, cudaStream_t st) {
+  const size_t need = fp16_operands_workspace_bytes(p, bwd);
+  if (p.workspace == nullptr || p.workspace_bytes < need) {
+    set_error("hstu_attn_%s: workspace of %zu bytes required (got %zu)", bwd ? "bwd" : "fwd", need, p.workspace_bytes);
+    return HSTU_ERR_WORKSPACE;
+  }
+  uint8_t* ws = reinterpret_cast<uint8_t*>(p.workspace);
+  const size_t amax_bytes = (size_t)p.batch * p.heads * kAmaxSlots * sizeof(uint32_t);
+  const size_t copy = align256((size_t)p.total_rows * p.heads * kPreD * sizeof(__half));
+  PreParams pp;
+  memset(&pp, 0, sizeof(pp));
+  pp.amax = reinterpret_cast<uint32_t*>(ws);
+  const void* src[kAmaxSlots] = {p.q, p.k, p.v, p.dout};
+  const long long rs[kAmaxSlots] = {p.q_row_stride, p.k_row_stride, p.v_row_stride, p.do_row_stride};
+  const long long hs[kAmaxSlots] = {p.q_head_stride, p.k_head_stride, p.v_head_stride, p.do_head_stride};
+  pp.nops = bwd ? 4 : 3;
+  for (int o = 0; o < pp.nops; ++o) {
+    pp.op[o].src = reinterpret_cast<const uint16_t*>(src[o]);
+    pp.op[o].row_stride = rs[o];
+    pp.op[o].head_stride = hs[o];
+    pp.op[o].dst = reinterpret_cast<__half*>(ws + align256(amax_bytes) + o * copy);
+    out->copy[o] = pp.op[o].dst;
+  }
+  out->amax = pp.amax;
+  pp.seq_offsets = p.seq_offsets;
+  pp.offsets_i64 = p.offsets_are_i64;
+  pp.max_seq_len = p.max_seq_len;
+  pp.heads = p.heads;
+  pp.alpha = p.alpha;
+  HSTU_CUDA_OK(cudaMemsetAsync(pp.amax, 0, amax_bytes, st));
+  if (p.batch == 0 || p.max_seq_len <= 0) return 0;
+  const dim3 grid((p.max_seq_len + kPreRows - 1) / kPreRows, p.heads, p.batch);
+  fp16_operands_amax_kernel<<<grid, kPreThreads, 0, st>>>(pp);
+  HSTU_CUDA_OK(cudaGetLastError());
+  fp16_operands_convert_kernel<<<grid, kPreThreads, 0, st>>>(pp);
+  HSTU_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace hstu

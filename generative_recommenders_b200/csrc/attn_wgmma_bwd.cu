@@ -19,7 +19,9 @@
 // Each warpgroup waits for its own MMAs before the next elementwise step (an MMA batch left in flight across it makes ptxas
 // serialise the batch); a Q_j / dO_j stage is released as soon as dV / dK of tile j have completed.
 // P and dS are 16-bit operands of the input format: fp16, or for bf16 inputs a hi + lo pair of bf16 operands (wgmma.cuh,
-// Operand), so that their rounding stays inside the 1e-3 parity budget whatever the scale of dO.
+// Operand), so that their rounding stays inside the 1e-3 parity budget whatever the scale of dO.  bf16 inputs at d = 32 run
+// the fp16 kernels below on exactly scaled fp16 copies of q, k, v, dO with scaled fp16 P and dS (`amax`,
+// attn_fp16_operands.cuh); their epilogues undo the scales and write bf16.
 //
 //
 // d = 32 runs two kernels instead, with no atomics and no per-tile coupling between the warpgroups (DESIGN.md 3.2):
@@ -35,6 +37,7 @@
 // kernel dQ is accumulated in fp32, not in the input dtype (triton_attention_utils.py:47-60).
 #include <string.h>
 
+#include "attn_fp16_operands.cuh"
 #include "common.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
@@ -60,6 +63,25 @@ struct alignas(64) BwdParams {
   float alpha_half;
   float dv_scale;  // 1 / N
   float dk_scale;  // alpha / (2 N): dS^T holds 2 dS N / alpha
+  const uint32_t* amax;  // fp16 kernels on scaled copies of bf16 inputs: [B, H, 4] amax bits (attn_fp16_operands.cuh); else null
+};
+
+// Scalars of the d = 32 kernels on scaled fp16 operands (identities for unscaled inputs): the score accumulators hold
+// 2^(e_q + e_k) S and 2^(e_v + e_o) dP; P and 2 dS N / alpha are formed as 2^e_p P and 2^e_s (2 dS N / alpha).
+struct BwdScales {
+  float c_s = 0.f, c_p = 1.f, c_d = 1.f;  // alpha / 2 * 2^-(e_q + e_k), 2^e_p, 2^(e_s - e_v - e_o)
+  int e_dv = 0, e_dk = 0, e_dq = 0;       // epilogue exponents: -(e_p + e_o), -(e_s + e_q), -(e_s + e_k)
+  __device__ __forceinline__ BwdScales(const BwdParams& p, int b, int h, int d) {
+    c_s = p.alpha_half;
+    if (p.amax == nullptr) return;
+    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, 2.f * p.alpha_half, d);
+    c_s = ldexpf(p.alpha_half, -(ex.q + ex.k));
+    c_p = pow2f(ex.p);
+    c_d = pow2f(ex.s - ex.v - ex.o);
+    e_dv = -(ex.p + ex.o);
+    e_dk = -(ex.s + ex.q);
+    e_dq = -(ex.s + ex.k);
+  }
 };
 
 // FUSED_DQ: the key-tile kernel also computes dQ (dS buffers in shared memory); without it the layout ends after the ring
@@ -181,6 +203,8 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   // keys of this tile that every query row >= q_full_from may attend (fast mask): all of them are history keys below the row
   const bool keys_hist = !msk.has_tgt || n0 + Cfg::BKV <= msk.max_id;
 
+  constexpr bool kScaled = !BF16 && !FUSED_DQ;  // the d = 32 dK / dV kernel also runs bf16 inputs on fp16 copies
+  const BwdScales sc(p, b, h, D);
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int e = 0; e < D / 2; ++e) dv[e] = dk[e] = 0.f;
@@ -236,10 +260,11 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     for (int nb = 0; nb < BQ / 8; ++nb)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float x = s[nb * 4 + e] * p.alpha_half;
+        const float x = s[nb * 4 + e] * (kScaled ? sc.c_s : p.alpha_half), xp = kScaled ? x * sc.c_p : x;
         const float t = tanh_approx(x);
         const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
-        float pv = __fmaf_rn(x, t, x), dsv = __fmaf_rn(dp[nb * 4 + e], g2, dp[nb * 4 + e]);
+        float pv = __fmaf_rn(xp, t, xp), dsv = __fmaf_rn(dp[nb * 4 + e], g2, dp[nb * 4 + e]);
+        if (kScaled) dsv *= sc.c_d;
         if (!full) {
           const int kj = k_base + (e >> 1) * 8, qi = q0 + nb * 8 + 2 * t4 + (e & 1);
           const bool v = kj < len && qi < len && mask_valid(msk, qi, kj);
@@ -369,10 +394,15 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
       uint16_t* vrow = reinterpret_cast<uint16_t*>(p.dv) + (row0 + kj) * p.dv_row_stride + (long long)h * p.dv_head_stride + 2 * t4;
 #pragma unroll
       for (int nb = 0; nb < D / 8; ++nb) {
-        const float k0 = dk[nb * 4 + hh * 2] * p.dk_scale, k1 = dk[nb * 4 + hh * 2 + 1] * p.dk_scale;
-        const float v0 = dv[nb * 4 + hh * 2] * p.dv_scale, v1 = dv[nb * 4 + hh * 2 + 1] * p.dv_scale;
-        *reinterpret_cast<uint32_t*>(krow + nb * 8) = BF16 ? pack_bf16x2(k0, k1) : pack_f16x2(k0, k1);
-        *reinterpret_cast<uint32_t*>(vrow + nb * 8) = BF16 ? pack_bf16x2(v0, v1) : pack_f16x2(v0, v1);
+        float k0 = dk[nb * 4 + hh * 2] * p.dk_scale, k1 = dk[nb * 4 + hh * 2 + 1] * p.dk_scale;
+        float v0 = dv[nb * 4 + hh * 2] * p.dv_scale, v1 = dv[nb * 4 + hh * 2 + 1] * p.dv_scale;
+        if (kScaled) {
+          k0 = scalbnf(k0, sc.e_dk), k1 = scalbnf(k1, sc.e_dk);
+          v0 = scalbnf(v0, sc.e_dv), v1 = scalbnf(v1, sc.e_dv);
+        }
+        const bool out_bf16 = BF16 || p.amax != nullptr;
+        *reinterpret_cast<uint32_t*>(krow + nb * 8) = out_bf16 ? pack_bf16x2(k0, k1) : pack_f16x2(k0, k1);
+        *reinterpret_cast<uint32_t*>(vrow + nb * 8) = out_bf16 ? pack_bf16x2(v0, v1) : pack_f16x2(v0, v1);
       }
     }
   }
@@ -496,6 +526,7 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
   const bool fast = msk.fast != 0;
   const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
 
+  const BwdScales sc(p, b, h, D);
   float dq[D / 2];
 #pragma unroll
   for (int e = 0; e < D / 2; ++e) dq[e] = 0.f;
@@ -545,10 +576,11 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
     for (int nb = 0; nb < BN / 8; ++nb)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float x = s[nb * 4 + e] * p.alpha_half;
+        const float x = s[nb * 4 + e] * sc.c_s;
         const float t = tanh_approx(x);
         const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
         float dsv = __fmaf_rn(dp[nb * 4 + e], g2, dp[nb * 4 + e]);
+        if (!BF16) dsv *= sc.c_d;
         if (!full) {
           const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
           dsv = (kj < len && mask_valid(msk, qi, kj)) ? dsv : 0.f;
@@ -588,8 +620,9 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
       uint16_t* qrow = reinterpret_cast<uint16_t*>(p.dq) + (row0 + qi) * p.dq_row_stride + (long long)h * p.dq_head_stride;
 #pragma unroll
       for (int nb = 0; nb < D / 8; ++nb) {
-        const float a = dq[nb * 4 + hh * 2] * p.dk_scale, c = dq[nb * 4 + hh * 2 + 1] * p.dk_scale;
-        *reinterpret_cast<uint32_t*>(qrow + nb * 8 + 2 * t4) = BF16 ? pack_bf16x2(a, c) : pack_f16x2(a, c);
+        float a = dq[nb * 4 + hh * 2] * p.dk_scale, c = dq[nb * 4 + hh * 2 + 1] * p.dk_scale;
+        if (!BF16) a = scalbnf(a, sc.e_dq), c = scalbnf(c, sc.e_dq);
+        *reinterpret_cast<uint32_t*>(qrow + nb * 8 + 2 * t4) = (BF16 || p.amax != nullptr) ? pack_bf16x2(a, c) : pack_f16x2(a, c);
       }
     }
   }
@@ -642,26 +675,38 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd) {
 // d = 32: dK / dV and dQ in two kernels, without atomics or workspace; larger d: the fused kernel (DESIGN.md 3.2)
 static constexpr bool split_dq(int d) { return d == 32; }
 
+// bf16 at d = 32: the fp16 kernels on exactly scaled copies (attn_fp16_operands.cu)
+static bool fp16_copies(const hstu_attn_params& p) { return p.dtype == HSTU_BF16 && p.dqk == 32; }
+
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd) {
+  if (fp16_copies(p)) return fp16_operands_workspace_bytes(p, bwd);
   if (!bwd || split_dq(p.dqk)) return 0;
   return (size_t)p.total_rows * p.heads * p.dqk * sizeof(float);  // fp32 dQ accumulator [L, H, D]
 }
 
+// f16: the scaled fp16 copies of bf16 inputs (the kernels are then the fp16 ones), or null
 template <int D, bool BF16>
-static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
+static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp16Operands* f16 = nullptr) {
   constexpr bool kSplit = split_dq(D);
   using Cfg = BwdCfg<D, !kSplit>;
-  const size_t need = wgmma_workspace_bytes(p, true);
+  const size_t need = f16 ? 0 : wgmma_workspace_bytes(p, true);
   if (need > 0 && (p.workspace == nullptr || p.workspace_bytes < need)) {
     set_error("hstu_attn_bwd: workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
     return HSTU_ERR_WORKSPACE;
   }
+  // operands the kernels read: the inputs, or their contiguous fp16 copies
+  const void* src[4] = {p.q, p.k, p.v, p.dout};
+  long long rs[4] = {p.q_row_stride, p.k_row_stride, p.v_row_stride, p.do_row_stride};
+  long long hs[4] = {p.q_head_stride, p.k_head_stride, p.v_head_stride, p.do_head_stride};
+  if (f16)
+    for (int i = 0; i < 4; ++i) src[i] = f16->copy[i], rs[i] = (long long)p.heads * D, hs[i] = D;
   BwdParams bp;
   memset(&bp, 0, sizeof(bp));
-  if (int e = make_tmap_rows_heads(&bp.tmQ, p.q, p.total_rows, p.heads, D, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BQ)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmK, p.k, p.total_rows, p.heads, D, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BKV)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmV, p.v, p.total_rows, p.heads, D, p.v_row_stride, p.v_head_stride, Cfg::BOX_COLS, Cfg::BKV)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmDO, p.dout, p.total_rows, p.heads, D, p.do_row_stride, p.do_head_stride, Cfg::BOX_COLS, Cfg::BQ)) return e;
+  if (f16) bp.amax = f16->amax;
+  if (int e = make_tmap_rows_heads(&bp.tmQ, src[0], p.total_rows, p.heads, D, rs[0], hs[0], Cfg::BOX_COLS, Cfg::BQ)) return e;
+  if (int e = make_tmap_rows_heads(&bp.tmK, src[1], p.total_rows, p.heads, D, rs[1], hs[1], Cfg::BOX_COLS, Cfg::BKV)) return e;
+  if (int e = make_tmap_rows_heads(&bp.tmV, src[2], p.total_rows, p.heads, D, rs[2], hs[2], Cfg::BOX_COLS, Cfg::BKV)) return e;
+  if (int e = make_tmap_rows_heads(&bp.tmDO, src[3], p.total_rows, p.heads, D, rs[3], hs[3], Cfg::BOX_COLS, Cfg::BQ)) return e;
   bp.seq_offsets = p.seq_offsets;
   bp.num_targets = p.num_targets;
   bp.dk = p.dk;
@@ -691,10 +736,10 @@ static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
     HSTU_CUDA_OK(cudaGetLastError());
     // the dQ kernel tiles 128 query rows and 64 key rows
     using QC = DqCfg<D>;
-    if (int e = make_tmap_rows_heads(&bp.tmQ, p.q, p.total_rows, p.heads, D, p.q_row_stride, p.q_head_stride, QC::BOX_COLS, QC::BM)) return e;
-    if (int e = make_tmap_rows_heads(&bp.tmK, p.k, p.total_rows, p.heads, D, p.k_row_stride, p.k_head_stride, QC::BOX_COLS, QC::BN)) return e;
-    if (int e = make_tmap_rows_heads(&bp.tmV, p.v, p.total_rows, p.heads, D, p.v_row_stride, p.v_head_stride, QC::BOX_COLS, QC::BN)) return e;
-    if (int e = make_tmap_rows_heads(&bp.tmDO, p.dout, p.total_rows, p.heads, D, p.do_row_stride, p.do_head_stride, QC::BOX_COLS, QC::BM)) return e;
+    if (int e = make_tmap_rows_heads(&bp.tmQ, src[0], p.total_rows, p.heads, D, rs[0], hs[0], QC::BOX_COLS, QC::BM)) return e;
+    if (int e = make_tmap_rows_heads(&bp.tmK, src[1], p.total_rows, p.heads, D, rs[1], hs[1], QC::BOX_COLS, QC::BN)) return e;
+    if (int e = make_tmap_rows_heads(&bp.tmV, src[2], p.total_rows, p.heads, D, rs[2], hs[2], QC::BOX_COLS, QC::BN)) return e;
+    if (int e = make_tmap_rows_heads(&bp.tmDO, src[3], p.total_rows, p.heads, D, rs[3], hs[3], QC::BOX_COLS, QC::BM)) return e;
     auto kdq = attn_bwd_dq_wgmma_kernel<D, BF16>;
     HSTU_CUDA_OK(cudaFuncSetAttribute(kdq, cudaFuncAttributeMaxDynamicSharedMemorySize, QC::SMEM_BYTES));
     kdq<<<dim3((p.max_seq_len + QC::BM - 1) / QC::BM, p.heads, p.batch), kBwdThreads, QC::SMEM_BYTES, st>>>(bp);
@@ -719,7 +764,12 @@ static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st) {
   const bool bf = p.dtype == HSTU_BF16;
   switch (p.dqk) {
-    case 32: return bf ? launch_bwd_wgmma<32, true>(p, st) : launch_bwd_wgmma<32, false>(p, st);
+    case 32: {  // bf16: the fp16 kernels on exactly scaled copies (DESIGN.md 3.0)
+      if (!bf) return launch_bwd_wgmma<32, false>(p, st);
+      Fp16Operands f16;
+      if (int e = fp16_operands_prepass(p, true, &f16, st)) return e;
+      return launch_bwd_wgmma<32, false>(p, st, &f16);
+    }
     case 64: return bf ? launch_bwd_wgmma<64, true>(p, st) : launch_bwd_wgmma<64, false>(p, st);
     case 128: return bf ? launch_bwd_wgmma<128, true>(p, st) : launch_bwd_wgmma<128, false>(p, st);
   }

@@ -16,7 +16,8 @@
 // 256-thread block.
 // P is a 16-bit MMA operand of the same format as V (wgmma takes one format for A and B): fp16 for fp16 inputs, and for
 // bf16 inputs a hi + lo pair of bf16 operands multiplied twice (wgmma.cuh, Operand), so that its rounding stays well inside
-// the 1e-3 parity budget.  The 1/N factor of the reference is applied once in the epilogue (registers -> global, rows past
+// the 1e-3 parity budget.  bf16 inputs at d = 32 instead run the fp16 kernel on exactly scaled fp16 copies of q, k, v with
+// a scaled fp16 P (`amax`, attn_fp16_operands.cuh); its epilogue undoes the scales and writes bf16.  The 1/N factor of the reference is applied once in the epilogue (registers -> global, rows past
 // the sequence end are not written).  Rows past the sequence end that a TMA box drags in are masked out of P, and zeroed in the
 // V stage of the one key tile that crosses the end (zero_tile_rows), since P = 0 does not neutralise a NaN or Inf in V.
 //
@@ -24,6 +25,7 @@
 // ops/triton/triton_hstu_attention.py:517-543 (loop bounds from the mask) but is derived from common.cuh's ranges.
 #include <string.h>
 
+#include "attn_fp16_operands.cuh"
 #include "common.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
@@ -42,6 +44,8 @@ struct alignas(64) FwdParams {
   int win, min_full, ctx;
   float alpha_half;  // alpha / 2
   float inv_n;       // 1 / max_seq_len
+  const uint32_t* amax;  // fp16 kernel on scaled copies of bf16 inputs: [B, H, 4] amax bits (attn_fp16_operands.cuh); else null
+  int heads;
 };
 
 template <int D>
@@ -147,6 +151,16 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
   const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
   const bool fast = msk.fast != 0;
   const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
+  // scaled fp16 operands: S holds 2^(e_q + e_k) S, P is formed as 2^e_p P and O holds 2^(e_p + e_v) O
+  constexpr bool kScaled = !BF16 && D == 32;  // the only instantiation that runs bf16 inputs on fp16 copies
+  float c_s = p.alpha_half, c_p = 1.f;
+  int e_out = 0;
+  if (kScaled && p.amax != nullptr) {
+    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, 2.f * p.alpha_half, D);
+    c_s = ldexpf(p.alpha_half, -(ex.q + ex.k));
+    c_p = pow2f(ex.p);
+    e_out = -(ex.p + ex.v);
+  }
 
   float o[D / 2];
 #pragma unroll
@@ -186,8 +200,8 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
     for (int nb = 0; nb < BN / 8; ++nb)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float x = s[nb * 4 + e] * p.alpha_half;
-        float pv = __fmaf_rn(x, tanh_approx(x), x);  // silu(2x) = x (1 + tanh x)
+        const float x = s[nb * 4 + e] * c_s, xp = kScaled ? x * c_p : x;
+        float pv = __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
         if (!full) {
           const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
           pv = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
@@ -237,6 +251,7 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
   }
 
   // ---------------- epilogue: O * 1/N -> global ----------------
+  const bool out_bf16 = BF16 || p.amax != nullptr;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int qi = q_base + hh * 8;
@@ -244,8 +259,9 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
       uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (row0 + qi) * p.o_row_stride + (long long)h * p.o_head_stride;
 #pragma unroll
       for (int nb = 0; nb < D / 8; ++nb) {
-        const float a = o[nb * 4 + hh * 2] * p.inv_n, c = o[nb * 4 + hh * 2 + 1] * p.inv_n;
-        *reinterpret_cast<uint32_t*>(orow + nb * 8 + 2 * t4) = BF16 ? pack_bf16x2(a, c) : pack_f16x2(a, c);
+        float a = o[nb * 4 + hh * 2] * p.inv_n, c = o[nb * 4 + hh * 2 + 1] * p.inv_n;
+        if (kScaled) a = scalbnf(a, e_out), c = scalbnf(c, e_out);
+        *reinterpret_cast<uint32_t*>(orow + nb * 8 + 2 * t4) = out_bf16 ? pack_bf16x2(a, c) : pack_f16x2(a, c);
       }
     }
   }
@@ -279,14 +295,24 @@ bool wgmma_fwd_supported(const hstu_attn_params& p) {
   return is_sm90();
 }
 
+// f16: the scaled fp16 copies of bf16 inputs (the kernel is then the fp16 one), or null
 template <int D, bool BF16>
-static int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
+static int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp16Operands* f16 = nullptr) {
   using Cfg = FwdCfg<D>;
   FwdParams fp;
   memset(&fp, 0, sizeof(fp));
-  if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, p.total_rows, p.heads, D, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BM)) return e;
-  if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, D, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
-  if (int e = make_tmap_rows_heads(&fp.tmV, p.v, p.total_rows, p.heads, D, p.v_row_stride, p.v_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
+  const long long crs = (long long)p.heads * D, chs = D;  // strides of the contiguous copies
+  if (f16) {
+    if (int e = make_tmap_rows_heads(&fp.tmQ, f16->copy[0], p.total_rows, p.heads, D, crs, chs, Cfg::BOX_COLS, Cfg::BM)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmK, f16->copy[1], p.total_rows, p.heads, D, crs, chs, Cfg::BOX_COLS, Cfg::BN)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmV, f16->copy[2], p.total_rows, p.heads, D, crs, chs, Cfg::BOX_COLS, Cfg::BN)) return e;
+    fp.amax = f16->amax;
+  } else {
+    if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, p.total_rows, p.heads, D, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BM)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, D, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmV, p.v, p.total_rows, p.heads, D, p.v_row_stride, p.v_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
+  }
+  fp.heads = p.heads;
   fp.seq_offsets = p.seq_offsets;
   fp.num_targets = p.num_targets;
   fp.out = p.out;
@@ -311,7 +337,12 @@ static int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st) {
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st) {
   const bool bf = p.dtype == HSTU_BF16;
   switch (p.dqk) {
-    case 32: return bf ? launch_fwd_wgmma<32, true>(p, st) : launch_fwd_wgmma<32, false>(p, st);
+    case 32: {  // bf16: the fp16 kernel on exactly scaled copies (DESIGN.md 3.0)
+      if (!bf) return launch_fwd_wgmma<32, false>(p, st);
+      Fp16Operands f16;
+      if (int e = fp16_operands_prepass(p, false, &f16, st)) return e;
+      return launch_fwd_wgmma<32, false>(p, st, &f16);
+    }
     case 64: return bf ? launch_fwd_wgmma<64, true>(p, st) : launch_fwd_wgmma<64, false>(p, st);
     case 128: return bf ? launch_fwd_wgmma<128, true>(p, st) : launch_fwd_wgmma<128, false>(p, st);
     case 256: return bf ? launch_fwd_wgmma<256, true>(p, st) : launch_fwd_wgmma<256, false>(p, st);

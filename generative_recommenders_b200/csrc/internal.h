@@ -18,6 +18,14 @@ size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
 
+// attn_fp16_operands.cu: per (sequence, head) amax and exactly scaled fp16 copies of the bf16 d = 32 operands
+struct Fp16Operands {
+  const unsigned int* amax;  // [B, H, 4] bits of max |q|, |k|, |v|, |dO| (attn_fp16_operands.cuh)
+  const void* copy[4];       // fp16 [L, H, 32] copies of q, k, v, dO (dO: backward only)
+};
+size_t fp16_operands_workspace_bytes(const hstu_attn_params& p, bool bwd);
+int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out, cudaStream_t st);
+
 // norm.cu
 int layer_norm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, long long n, int D,
                    long long xs, long long ys, float eps, int dtype, int swish, bool rms, cudaStream_t st);

@@ -82,7 +82,8 @@ def cuda_hstu_attention_fwd(
     ws = _workspace(p, False, dev)
     with torch.cuda.device(dev), _lib.timed("attn_fwd", dev):
         _lib.check(_lib.lib().hstu_attn_fwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_fwd")
-    _lib.note_launch(1)
+    # bf16 at d = 32: amax and convert kernels before the attention kernel (the forward's only workspace: the fp16 copies)
+    _lib.note_launch(3 if ws is not None else 1)
     del ws, keep
     return out
 
@@ -116,8 +117,9 @@ def cuda_hstu_attention_bwd(
     ws = _workspace(p, True, dev)
     with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
         _lib.check(_lib.lib().hstu_attn_bwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_bwd")
-    # wgmma path: dK/dV kernel + dQ kernel (d = 32) or main kernel + dQ convert; generic path: dK/dV kernel + dQ kernel
-    _lib.note_launch(2)
+    # wgmma path: dK/dV kernel + dQ kernel (d = 32, after the amax and convert kernels for bf16) or main kernel + dQ convert;
+    # generic path: dK/dV kernel + dQ kernel
+    _lib.note_launch(4 if ws is not None and p.dtype == _lib.BF16 and p.dqk == 32 else 2)
     del ws, keep
 
 
