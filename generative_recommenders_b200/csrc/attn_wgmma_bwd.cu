@@ -254,26 +254,44 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     fence_regs(s);
     fence_regs(dp);
 
-    // p = x sig(x) and 2 dS = dP (1 + g2) from one tanh (h = alpha s / 2, t = tanh h, p = h (1 + t), g2 = t + h (1 - t^2))
-    const bool full = fast && keys_hist && n0 + Cfg::BKV <= q0 && q0 + BQ <= len;  // tile-uniform: every pair valid
+    // p = x sig(x) and 2 dS = dP (1 + g2) from one tanh (h = alpha s / 2, t = tanh h, p = h (1 + t), g2 = t + h (1 - t^2)).
+    // The mask case is chosen once per tile, outside the score loops, so that ptxas can overlap the tanh of independent
+    // scores (as in the forward).  `v`: the pair is valid.
+    auto score = [&](int n, bool v) {
+      const float x = s[n] * (kScaled ? sc.c_s : p.alpha_half), xp = kScaled ? x * sc.c_p : x;
+      const float t = tanh_approx(x);
+      const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
+      const float pv = __fmaf_rn(xp, t, xp);
+      float dsv = __fmaf_rn(dp[n], g2, dp[n]);
+      if (kScaled) dsv *= sc.c_d;
+      s[n] = v ? pv : 0.f;
+      dp[n] = v ? dsv : 0.f;
+    };
+    if (fast && keys_hist && n0 + Cfg::BKV <= q0 && q0 + BQ <= len) {  // tile-uniform: every pair valid
 #pragma unroll
-    for (int nb = 0; nb < BQ / 8; ++nb)
+      for (int n = 0; n < BQ / 2; ++n) score(n, true);
+    } else if (fast) {
+      // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limit of each query column computed once
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float x = s[nb * 4 + e] * (kScaled ? sc.c_s : p.alpha_half), xp = kScaled ? x * sc.c_p : x;
-        const float t = tanh_approx(x);
-        const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
-        float pv = __fmaf_rn(xp, t, xp), dsv = __fmaf_rn(dp[nb * 4 + e], g2, dp[nb * 4 + e]);
-        if (kScaled) dsv *= sc.c_d;
-        if (!full) {
-          const int kj = k_base + (e >> 1) * 8, qi = q0 + nb * 8 + 2 * t4 + (e & 1);
-          const bool v = kj < len && qi < len && mask_valid(msk, qi, kj);
-          pv = v ? pv : 0.f;
-          dsv = v ? dsv : 0.f;
+      for (int nb = 0; nb < BQ / 8; ++nb)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int qi = q0 + nb * 8 + 2 * t4 + c, lim = msk.has_tgt ? min(qi, msk.max_id) : qi;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int kj = k_base + hh * 8;
+            score(nb * 4 + hh * 2 + c, kj < len && qi < len && (kj < lim || kj == qi));
+          }
         }
-        s[nb * 4 + e] = pv;
-        dp[nb * 4 + e] = dsv;
-      }
+    } else {
+#pragma unroll
+      for (int nb = 0; nb < BQ / 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int kj = k_base + (e >> 1) * 8, qi = q0 + nb * 8 + 2 * t4 + (e & 1);
+          score(nb * 4 + e, kj < len && qi < len && mask_valid(msk, qi, kj));
+        }
+    }
     if constexpr (FUSED_DQ) {
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
@@ -570,23 +588,42 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
     release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i);
     __syncwarp();
 
-    // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2
-    const bool full = n0 + BN <= full_lim;  // tile-uniform
+    // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2.  The mask case is chosen once per
+    // tile, outside the score loops, so that ptxas can overlap the tanh of independent scores (as in the forward).
+    auto dscore = [&](int n) {
+      const float x = s[n] * sc.c_s;
+      const float t = tanh_approx(x);
+      const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
+      float dsv = __fmaf_rn(dp[n], g2, dp[n]);
+      if (!BF16) dsv *= sc.c_d;
+      return dsv;
+    };
+    if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
 #pragma unroll
-    for (int nb = 0; nb < BN / 8; ++nb)
+      for (int n = 0; n < BN / 2; ++n) dp[n] = dscore(n);
+    } else if (fast) {
+      // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limits of the thread's two rows hoisted
+      int lim[2];
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float x = s[nb * 4 + e] * sc.c_s;
-        const float t = tanh_approx(x);
-        const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
-        float dsv = __fmaf_rn(dp[nb * 4 + e], g2, dp[nb * 4 + e]);
-        if (!BF16) dsv *= sc.c_d;
-        if (!full) {
+      for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
+#pragma unroll
+      for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
           const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          dsv = (kj < len && mask_valid(msk, qi, kj)) ? dsv : 0.f;
+          const float dsv = dscore(nb * 4 + e);
+          dp[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? dsv : 0.f;
         }
-        dp[nb * 4 + e] = dsv;
-      }
+    } else {
+#pragma unroll
+      for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+          const float dsv = dscore(nb * 4 + e);
+          dp[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? dsv : 0.f;
+        }
+    }
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk) {
 #pragma unroll

@@ -195,19 +195,38 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
     const int st = i % NST;
     const bool next = i + 1 < T;
     const int n0 = (t0 + i) * BN;
-    const bool full = n0 + BN <= full_lim;  // tile-uniform
+    // P = silu(alpha S) * mask.  The mask case is chosen once per tile, outside the score loops, so that each loop is one
+    // basic block and ptxas can overlap the tanh of independent scores instead of waiting out each one in turn.
+    auto silu = [&](int n) {
+      const float x = s[n] * c_s, xp = kScaled ? x * c_p : x;
+      return __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
+    };
+    if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
 #pragma unroll
-    for (int nb = 0; nb < BN / 8; ++nb)
+      for (int n = 0; n < BN / 2; ++n) s[n] = silu(n);
+    } else if (fast) {
+      // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limits of the thread's two rows hoisted
+      int lim[2];
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float x = s[nb * 4 + e] * c_s, xp = kScaled ? x * c_p : x;
-        float pv = __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
-        if (!full) {
+      for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
+#pragma unroll
+      for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
           const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          pv = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
+          const float pv = silu(nb * 4 + e);
+          s[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? pv : 0.f;
         }
-        s[nb * 4 + e] = pv;
-      }
+    } else {
+#pragma unroll
+      for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+          const float pv = silu(nb * 4 + e);
+          s[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
+        }
+    }
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk) {
       const Operand<BF16> x0(s[8 * kk + 0], s[8 * kk + 1]), x1(s[8 * kk + 2], s[8 * kk + 3]);
