@@ -37,7 +37,7 @@ class AttnParams(C.Structure):
         ("dq_head_stride", C.c_int64), ("dk_row_stride", C.c_int64), ("dk_head_stride", C.c_int64),
         ("dv_row_stride", C.c_int64), ("dv_head_stride", C.c_int64),
         ("pos_w", C.c_void_p), ("ts_w", C.c_void_p), ("timestamps", C.c_void_p), ("num_ts_buckets", C.c_int32),
-        ("reserved0", C.c_int32), ("dpos_w", C.c_void_p), ("dts_w", C.c_void_p),
+        ("deterministic", C.c_int32), ("dpos_w", C.c_void_p), ("dts_w", C.c_void_p),
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
     ]
 

@@ -38,6 +38,7 @@ static int validate_attn(const hstu_attn_params* p, bool bwd) {
   }
   if (p->ts_w) HSTU_CHECK_ARG(p->timestamps != nullptr, "ts_w given without timestamps");
   HSTU_CHECK_ARG(p->impl >= HSTU_IMPL_AUTO && p->impl <= HSTU_IMPL_UMMA, "bad impl %d", p->impl);
+  HSTU_CHECK_ARG(p->deterministic == 0 || p->deterministic == 1, "deterministic must be 0 or 1 (got %d)", p->deterministic);
   return 0;
 }
 
@@ -57,7 +58,14 @@ int bind_device(const void* ptr) {
   return 0;
 }
 
+// A deterministic backward takes the same route as any other: the wgmma kernels run their atomic-free split path
+// (attn_wgmma_bwd.cu), and the generic kernels have no atomics on q / k / v.
 static int select_impl(const hstu_attn_params* p, bool bwd) {
+  if (bwd && p->deterministic && (p->pos_w != nullptr || p->ts_w != nullptr)) {
+    set_error("deterministic backward with a relative bias is not supported: the dpos_w / dts_w gradients are added "
+              "with atomics");
+    return HSTU_ERR_UNSUPPORTED;
+  }
   const bool can = wgmma_supported(*p, bwd);
   if (p->impl == HSTU_IMPL_GENERIC) return HSTU_IMPL_GENERIC;
   if (p->impl == HSTU_IMPL_UMMA) {

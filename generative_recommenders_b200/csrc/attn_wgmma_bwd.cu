@@ -24,14 +24,18 @@
 // attn_fp16_operands.cuh); their epilogues undo the scales and write bf16.
 //
 //
-// d = 32 runs two kernels instead, with no atomics and no per-tile coupling between the warpgroups (DESIGN.md 3.2):
+// d = 32, and d = 64 / 128 when the caller asks for a deterministic backward (hstu_attn_params.deterministic), run two
+// kernels instead, with no atomics and no per-tile coupling between the warpgroups (DESIGN.md 3.2):
 //   attn_bwd_dkdv_wgmma_kernel  the kernel above without the dS buffers, the dS barrier and dQ: dK and dV only.
 //   attn_bwd_dq_wgmma_kernel    query-stationary, shaped like the forward: one CTA per (128-row query tile, head, sequence),
 //                               Q and dO resident, K and V streamed in 64-key tiles; it recomputes S = Q K^T and
 //                               dP = dO V^T, forms dS from one tanh and accumulates dQ += dS K in registers.  Its K / V ring
 //                               is refilled like the forward's, by the last warp to release a stage.
+// Every dq / dk / dv element is then summed by one thread in a fixed order, so the result is bitwise reproducible.
 // At d = 32 recomputing S and dP costs two MMA units per score against the eight that the whole backward issues, while the
-// elementwise work per score is the same; at larger d the recomputed MMAs weigh more and the fused kernel is kept.
+// elementwise work per score is the same; at larger d the recomputed MMAs weigh more and the fused kernel stays the default.
+// The split kernels run two CTAs per SM at d = 32 and one at d = 64 / 128 (their accumulators need more than 128
+// registers per thread there); bf16 at d = 64 / 128 keeps the hi + lo operand pairs.
 //
 // Reference math: ops/triton/triton_hstu_attention.py:995-1006,1222 and SURVEY.md appendix A; unlike the Triton
 // kernel dQ is accumulated in fp32, not in the input dtype (triton_attention_utils.py:47-60).
@@ -84,7 +88,12 @@ struct BwdScales {
   }
 };
 
-// FUSED_DQ: the key-tile kernel also computes dQ (dS buffers in shared memory); without it the layout ends after the ring
+// CTAs per SM of the split kernels: two at d = 32 (<= 128 registers per thread), one at d = 64 / 128
+constexpr int split_min_blocks(int d) { return d == 32 ? 2 : 1; }
+constexpr int kSmemPerSm = 232448;  // dynamic shared memory one CTA may use on sm_90
+
+// FUSED_DQ: the key-tile kernel also computes dQ (dS buffers in shared memory); without it the layout ends after the ring,
+// which then has four stages at every d (d = 128: 192 KB, one CTA per SM)
 template <int D, bool FUSED_DQ = true>
 struct BwdCfg {
   static constexpr int BKV = 128, BQ = 64;
@@ -95,7 +104,7 @@ struct BwdCfg {
   static constexpr int QD_BOX = BQ * SW;
   static constexpr int KV_BYTES = BKV * D * 2;
   static constexpr int QD_BYTES = BQ * D * 2;
-  static constexpr int STAGES = (D <= 32) ? 4 : (D == 64 ? 3 : 2);  // Q_j / dO_j ring depth
+  static constexpr int STAGES = (D <= 32 || !FUSED_DQ) ? 4 : (D == 64 ? 3 : 2);  // Q_j / dO_j ring depth
   static constexpr int DS_BYTES = BKV * BQ * 2;                      // one [128 kv][64 q] box, 128-byte swizzle
   static constexpr int DQN = D < 64 ? D : 64;                        // dQ columns per pass (one 128-byte box of K)
   static constexpr int OFF_K = 0;
@@ -105,7 +114,7 @@ struct BwdCfg {
   static constexpr int OFF_DS = OFF_DO + STAGES * QD_BYTES;          // [buffer 0/1][hi / lo]
   static constexpr int OFF_BAR = OFF_DS + (FUSED_DQ ? 4 * DS_BYTES : 0);
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+  static_assert(SMEM_BYTES * (FUSED_DQ ? 1 : split_min_blocks(D)) <= kSmemPerSm, "shared memory budget");
 };
 constexpr int kBwdThreads = 256;
 
@@ -203,7 +212,7 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   // keys of this tile that every query row >= q_full_from may attend (fast mask): all of them are history keys below the row
   const bool keys_hist = !msk.has_tgt || n0 + Cfg::BKV <= msk.max_id;
 
-  constexpr bool kScaled = !BF16 && !FUSED_DQ;  // the d = 32 dK / dV kernel also runs bf16 inputs on fp16 copies
+  constexpr bool kScaled = !BF16 && !FUSED_DQ && D == 32;  // the d = 32 dK / dV kernel also runs bf16 inputs on fp16 copies
   const BwdScales sc(p, b, h, D);
   float dv[D / 2], dk[D / 2];
 #pragma unroll
@@ -431,13 +440,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __
   bwd_key_tile<D, BF16, true>(p);
 }
 
-// two CTAs per SM (<= 128 registers per thread, 49 KB of shared memory at d = 32)
+// d = 32: two CTAs per SM (<= 128 registers per thread, 49 KB of shared memory)
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dkdv_wgmma_kernel(const __grid_constant__ BwdParams p) {
+__global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dkdv_wgmma_kernel(const __grid_constant__ BwdParams p) {
   bwd_key_tile<D, BF16, false>(p);
 }
 
-// ---------------- dQ, query-stationary (d = 32) ----------------
+// ---------------- dQ, query-stationary (split path) ----------------
 template <int D>
 struct DqCfg {
   static constexpr int BM = 128;  // query rows per CTA (two warpgroups of 64)
@@ -449,14 +458,14 @@ struct DqCfg {
   static constexpr int KV_BOX = BN * SW;
   static constexpr int Q_BYTES = BM * D * 2;
   static constexpr int KV_BYTES = BN * D * 2;
-  static constexpr int STAGES = 3;  // K / V ring depth
+  static constexpr int STAGES = 3;  // K / V ring depth (d = 128: 161 KB, one CTA per SM)
   static constexpr int OFF_Q = 0;
   static constexpr int OFF_DO = OFF_Q + Q_BYTES;
   static constexpr int OFF_K = OFF_DO + Q_BYTES;
   static constexpr int OFF_V = OFF_K + STAGES * KV_BYTES;
   static constexpr int OFF_BAR = OFF_V + STAGES * KV_BYTES;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static_assert(SMEM_BYTES <= 232448 / 2, "shared memory budget of two CTAs per SM");
+  static_assert(SMEM_BYTES * split_min_blocks(D) <= kSmemPerSm, "shared memory budget of split_min_blocks(D) CTAs per SM");
 };
 
 struct DqBars {
@@ -469,9 +478,10 @@ struct DqBars {
 // Per 64-key tile each warpgroup runs S = Q K^T and dP = dO V^T (A and B K-major), releases V, forms
 // 2 dS N / alpha = dP (1 + g2) * mask from one tanh, and runs dQ += dS K (A from registers, K read MN-major), then releases K.
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const __grid_constant__ BwdParams p) {
+__global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dq_wgmma_kernel(const __grid_constant__ BwdParams p) {
   using Cfg = DqCfg<D>;
   constexpr int SW = Cfg::SW, BN = Cfg::BN, NST = Cfg::STAGES;
+  constexpr bool kScaled = !BF16 && D == 32;  // also runs bf16 inputs on scaled fp16 copies
   const int b = blockIdx.z, h = blockIdx.y;
   const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
   const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
@@ -595,7 +605,7 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
       const float t = tanh_approx(x);
       const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
       float dsv = __fmaf_rn(dp[n], g2, dp[n]);
-      if (!BF16) dsv *= sc.c_d;
+      if (kScaled) dsv *= sc.c_d;
       return dsv;
     };
     if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
@@ -658,7 +668,7 @@ __global__ void __launch_bounds__(kBwdThreads, 2) attn_bwd_dq_wgmma_kernel(const
 #pragma unroll
       for (int nb = 0; nb < D / 8; ++nb) {
         float a = dq[nb * 4 + hh * 2] * p.dk_scale, c = dq[nb * 4 + hh * 2 + 1] * p.dk_scale;
-        if (!BF16) a = scalbnf(a, sc.e_dq), c = scalbnf(c, sc.e_dq);
+        if (kScaled) a = scalbnf(a, sc.e_dq), c = scalbnf(c, sc.e_dq);
         *reinterpret_cast<uint32_t*>(qrow + nb * 8 + 2 * t4) = (BF16 || p.amax != nullptr) ? pack_bf16x2(a, c) : pack_f16x2(a, c);
       }
     }
@@ -709,22 +719,23 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd) {
   return wgmma_bwd_supported(q);
 }
 
-// d = 32: dK / dV and dQ in two kernels, without atomics or workspace; larger d: the fused kernel (DESIGN.md 3.2)
-static constexpr bool split_dq(int d) { return d == 32; }
+// d = 32, or a deterministic backward: dK / dV and dQ in two kernels, without atomics or dQ workspace; otherwise the fused
+// kernel (DESIGN.md 3.2)
+static bool split_dq(const hstu_attn_params& p) { return p.dqk == 32 || p.deterministic != 0; }
 
 // bf16 at d = 32: the fp16 kernels on exactly scaled copies (attn_fp16_operands.cu)
 static bool fp16_copies(const hstu_attn_params& p) { return p.dtype == HSTU_BF16 && p.dqk == 32; }
 
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd) {
   if (fp16_copies(p)) return fp16_operands_workspace_bytes(p, bwd);
-  if (!bwd || split_dq(p.dqk)) return 0;
+  if (!bwd || split_dq(p)) return 0;
   return (size_t)p.total_rows * p.heads * p.dqk * sizeof(float);  // fp32 dQ accumulator [L, H, D]
 }
 
-// f16: the scaled fp16 copies of bf16 inputs (the kernels are then the fp16 ones), or null
-template <int D, bool BF16>
+// kSplit: the dK / dV and dQ kernels, else the fused kernel and the dQ convert.  f16: the scaled fp16 copies of bf16 inputs
+// (the kernels are then the fp16 ones), or null
+template <int D, bool BF16, bool kSplit>
 static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp16Operands* f16 = nullptr) {
-  constexpr bool kSplit = split_dq(D);
   using Cfg = BwdCfg<D, !kSplit>;
   const size_t need = f16 ? 0 : wgmma_workspace_bytes(p, true);
   if (need > 0 && (p.workspace == nullptr || p.workspace_bytes < need)) {
@@ -800,15 +811,20 @@ static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp
 
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st) {
   const bool bf = p.dtype == HSTU_BF16;
+  const bool split = split_dq(p);
   switch (p.dqk) {
     case 32: {  // bf16: the fp16 kernels on exactly scaled copies (DESIGN.md 3.0)
-      if (!bf) return launch_bwd_wgmma<32, false>(p, st);
+      if (!bf) return launch_bwd_wgmma<32, false, true>(p, st);
       Fp16Operands f16;
       if (int e = fp16_operands_prepass(p, true, &f16, st)) return e;
-      return launch_bwd_wgmma<32, false>(p, st, &f16);
+      return launch_bwd_wgmma<32, false, true>(p, st, &f16);
     }
-    case 64: return bf ? launch_bwd_wgmma<64, true>(p, st) : launch_bwd_wgmma<64, false>(p, st);
-    case 128: return bf ? launch_bwd_wgmma<128, true>(p, st) : launch_bwd_wgmma<128, false>(p, st);
+    case 64:
+      if (split) return bf ? launch_bwd_wgmma<64, true, true>(p, st) : launch_bwd_wgmma<64, false, true>(p, st);
+      return bf ? launch_bwd_wgmma<64, true, false>(p, st) : launch_bwd_wgmma<64, false, false>(p, st);
+    case 128:
+      if (split) return bf ? launch_bwd_wgmma<128, true, true>(p, st) : launch_bwd_wgmma<128, false, true>(p, st);
+      return bf ? launch_bwd_wgmma<128, true, false>(p, st) : launch_bwd_wgmma<128, false, false>(p, st);
   }
   set_error("wgmma backward: unsupported head dim %d", p.dqk);
   return HSTU_ERR_UNSUPPORTED;

@@ -95,8 +95,16 @@ def cuda_hstu_attention_bwd(
     min_full_attn_seq_len: int = 0, impl: int = _lib.IMPL_AUTO,
     bias: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
     dbias: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+    deterministic: Optional[bool] = None,
 ) -> None:
-    """Writes dq, dk, dv in place (last-dim stride 1 required; row/head strides arbitrary)."""
+    """Writes dq, dk, dv in place (last-dim stride 1 required; row/head strides arbitrary).
+
+    deterministic: dq / dk / dv bitwise reproducible from run to run (the wgmma backward then runs its atomic-free dK / dV
+    and dQ kernels at every head dim); None follows torch.are_deterministic_algorithms_enabled().  Not available with a
+    relative bias, whose table gradients are added with atomics.
+    """
+    if deterministic is None:
+        deterministic = torch.are_deterministic_algorithms_enabled()
     dev = _lib.require_cuda(dout, q, k, v, dq, dk, dv, seq_offsets, num_targets)
     q, k, v, dout = _prep(q, k, v, dout)
     for g in (dq, dk, dv):
@@ -113,12 +121,13 @@ def cuda_hstu_attention_bwd(
     p.dq_row_stride, p.dq_head_stride = dq.stride(0), dq.stride(1)
     p.dk_row_stride, p.dk_head_stride = dk.stride(0), dk.stride(1)
     p.dv_row_stride, p.dv_head_stride = dv.stride(0), dv.stride(1)
+    p.deterministic = int(bool(deterministic))
     keep = _fill_bias(p, bias, dbias)
     ws = _workspace(p, True, dev)
     with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
         _lib.check(_lib.lib().hstu_attn_bwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_bwd")
-    # wgmma path: dK/dV kernel + dQ kernel (d = 32, after the amax and convert kernels for bf16) or main kernel + dQ convert;
-    # generic path: dK/dV kernel + dQ kernel
+    # wgmma path: dK/dV kernel + dQ kernel (d = 32, after the amax and convert kernels for bf16; deterministic d = 64 / 128:
+    # no workspace, no memset, no convert) or main kernel + dQ convert; generic path: dK/dV kernel + dQ kernel
     _lib.note_launch(4 if ws is not None and p.dtype == _lib.BF16 and p.dqk == 32 else 2)
     del ws, keep
 
@@ -263,8 +272,9 @@ class _RelBiasAttentionFunction(torch.autograd.Function):
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
         dpos = torch.zeros(pos_w.shape, dtype=torch.float32, device=q.device)
         dts = torch.zeros(ts_w.shape, dtype=torch.float32, device=q.device) if ts_w is not None else None
+        # the bias-table gradients are added with atomics, so this backward is not reproducible whatever the global flag says
         cuda_hstu_attention_bwd(ctx.n, 1.0, dout, q, k, v, dq, dk, dv, seq_offsets, impl=_lib.IMPL_GENERIC,
-                                bias=(pos_w, ts_w, timestamps), dbias=(dpos, dts))
+                                bias=(pos_w, ts_w, timestamps), dbias=(dpos, dts), deterministic=False)
         return (None, dq, dk, dv, None, dpos.to(pos_w.dtype), None if dts is None else dts.to(ts_w.dtype), None)
 
 

@@ -7,15 +7,16 @@ already-loaded reference extension only if that one is absent -- a second defini
 routes them to libhstu_b200.so, so code written against `torch.ops.hstu.hstu_mha(...)` runs on H100 unchanged.
 
 Arguments this backend does not implement raise instead of being ignored: `attn_scale`, `q/k/v_descale` (fp8 paths).
-`deterministic=True` selects the CUDA-core backward (query-stationary dQ, no atomics / no reduce-add: bitwise reproducible);
-the default wgmma backward accumulates dQ with fp32 atomic adds whose order varies from run to run (fp32, ~1e-7 relative).
+`deterministic=True` (or `torch.use_deterministic_algorithms(True)`) makes the backward bitwise reproducible: the wgmma
+backward then runs its atomic-free dK / dV and dQ kernels, and shapes it does not cover run the generic kernels, which have
+no atomics either.  Otherwise the wgmma backward at d = 64 / 128 accumulates dQ with fp32 atomic adds whose order varies
+from run to run (fp32, ~1e-7 relative); at d = 32 it is atomic-free either way.
 `sort_by_length` / `sm_margin` are accepted and ignored (the kernels always schedule heavy tiles first and use every SM).
 """
 from typing import List, Optional
 
 import torch
 
-from . import _lib
 from .ops.hstu_attention import cuda_hstu_attention_bwd, cuda_hstu_attention_fwd
 
 _LIB = None
@@ -50,9 +51,13 @@ def _bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, causal, num
          min_full_attn_seq_len, contextual_seq_len, sort_by_length, deterministic, sm_margin) -> List[torch.Tensor]:
     _check(causal, seq_offsets, attn_scale, ())
     cuda_hstu_attention_bwd(int(max_seq_len), alpha, dout, q, k, v, dq, dk, dv, seq_offsets, num_targets, max_attn_len,
-                            contextual_seq_len, min_full_attn_seq_len,
-                            impl=_lib.IMPL_GENERIC if deterministic else _lib.IMPL_AUTO)
+                            contextual_seq_len, min_full_attn_seq_len, deterministic=_deterministic(deterministic))
     return [dq, dk, dv]
+
+
+def _deterministic(flag):
+    """deterministic=False of the schema leaves the choice to torch.use_deterministic_algorithms."""
+    return True if flag else None
 
 
 class _Mha(torch.autograd.Function):
@@ -69,7 +74,7 @@ class _Mha(torch.autograd.Function):
         max_seq_len, alpha, max_attn_len, min_full, ctx_len, deterministic = ctx.cfg
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
         cuda_hstu_attention_bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, num_targets, max_attn_len, ctx_len,
-                                min_full, impl=_lib.IMPL_GENERIC if deterministic else _lib.IMPL_AUTO)
+                                min_full, deterministic=_deterministic(deterministic))
         return None, None, dq, dk, dv, None, None, None, None, None, None
 
 

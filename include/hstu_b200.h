@@ -55,6 +55,8 @@ typedef enum hstu_status {
   HSTU_ERR_WORKSPACE = -4
 } hstu_status;
 
+/* Every implementation honours hstu_attn_params.deterministic: with it set, AUTO runs the backward on the atomic-free
+ * wgmma kernels where the shape allows (bf16/fp16, dqk == dv in {32, 64, 128}) and on the generic kernels otherwise. */
 typedef enum hstu_attn_impl {
   HSTU_IMPL_AUTO = 0,  /* wgmma/TMA kernels when the shape allows, else the generic kernels */
   HSTU_IMPL_GENERIC = 1, /* CUDA-core fp32-accumulate kernels: any dtype / head dim <= 256 / all mask options */
@@ -105,7 +107,8 @@ typedef struct hstu_attn_params {
   const float* ts_w;         /* [num_ts_buckets+1] or NULL */
   const int64_t* timestamps; /* [B, max_seq_len] or NULL */
   int32_t num_ts_buckets;
-  int32_t reserved0;
+  int32_t deterministic;     /* backward: 0 = fastest kernels (d = 64 / 128 on wgmma add dQ with fp32 atomics);
+                                1 = dq / dk / dv bitwise reproducible run to run (no relative bias: HSTU_ERR_UNSUPPORTED) */
   float* dpos_w;             /* backward: fp32 accumulators (atomically added), or NULL */
   float* dts_w;
   /* scratch */
@@ -116,11 +119,14 @@ typedef struct hstu_attn_params {
 const char* hstu_last_error(void);
 int hstu_abi_version(void);
 
-/* Bytes of scratch the call needs (is_backward: 0 fwd, 1 bwd).  Depends only on sizes/dtype/impl. */
+/* Bytes of scratch the call needs (is_backward: 0 fwd, 1 bwd).  Depends only on sizes/dtype/impl/deterministic. */
 size_t hstu_attn_workspace_bytes(const hstu_attn_params* p, int is_backward);
 int hstu_attn_fwd(const hstu_attn_params* p, void* cuda_stream);
 int hstu_attn_bwd(const hstu_attn_params* p, void* cuda_stream);
-/* Which implementation a call would dispatch to: returns HSTU_IMPL_GENERIC or HSTU_IMPL_UMMA (<0 on error). */
+/* Which implementation a call would dispatch to: returns HSTU_IMPL_GENERIC or HSTU_IMPL_UMMA (<0 on error).  A
+ * deterministic backward returns HSTU_IMPL_UMMA where the wgmma backward supports the shape (it then runs its atomic-free
+ * dK / dV and dQ kernels), else HSTU_IMPL_GENERIC; HSTU_ERR_UNSUPPORTED with a relative bias, or with impl forced to
+ * HSTU_IMPL_UMMA on a shape the wgmma backward does not support. */
 int hstu_attn_select_impl(const hstu_attn_params* p, int is_backward);
 
 /* ---- host-side helpers (pure CPU; used by the no-GPU tests to pin the mask / tile-skipping logic) ---- */

@@ -176,18 +176,19 @@ def run(T, d, seed, break_ds=False, straddle=True, break_zero=False):
     return _simulate({f"W{w}": W(w) for w in range(WARPS)}, B, rnd)
 
 
-DKDV_STAGES = 4  # BwdCfg<32, false>::STAGES
+DKDV_STAGES = 4  # BwdCfg<D, false>::STAGES (every d)
 
 
-def run_dkdv(T, seed, break_release=False, first_releaser=False, early_release=False, straddle=True, break_zero=False):
-    """attn_bwd_dkdv_wgmma_kernel (d = 32): the key-tile CTA of `run` without dS buffers, dS barrier or dQ; the warps meet at
-    the Q / dO ring and, with `straddle`, once at the named barrier after zeroing the rows of the last query tile that lie
-    past the sequence end.  Seeded breaks (each must be caught):
+def run_dkdv(T, seed, break_release=False, first_releaser=False, early_release=False, straddle=True, break_zero=False,
+             stages=DKDV_STAGES):
+    """attn_bwd_dkdv_wgmma_kernel: the key-tile CTA of `run` without dS buffers, dS barrier or dQ, with a ring of `stages`;
+    the warps meet at the Q / dO ring and, with `straddle`, once at the named barrier after zeroing the rows of the last
+    query tile that lie past the sequence end.  Seeded breaks (each must be caught):
       break_zero      no named barrier between that zeroing and the MMAs;
       break_release   the stage is refilled once four warps (one warpgroup's worth) have released it;
       first_releaser  the first warp to release the stage refills it;
       early_release   a warp releases Q_j / dO_j before the wait of the MMAs that read them."""
-    NST = DKDV_STAGES
+    NST = stages
     refill_at = 1 if first_releaser else WARPS // 2 if break_release else WARPS
     rnd = random.Random(seed)
     B = {"kv": Bar(1), "zb": Bar(WARPS)}

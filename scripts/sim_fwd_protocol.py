@@ -82,11 +82,12 @@ def run(T, d, seed, break_refill=False, first_releaser=False, early_release=Fals
     return _eng._simulate({f"W{w}": W(w) for w in range(WARPS)}, B, rnd)
 
 
-DQ_STAGES = 3  # DqCfg<32>::STAGES (csrc/attn_wgmma_bwd.cu)
+DQ_STAGES = 3  # DqCfg<D>::STAGES (csrc/attn_wgmma_bwd.cu, every d)
 
 
-def run_dq(T, seed, break_k_refill=False, first_releaser=False, early_release=False, straddle=True, break_zero=False):
-    """attn_bwd_dq_wgmma_kernel (d = 32): the forward's ring with Q and dO resident; S / dP read K and V and are waited for,
+def run_dq(T, seed, break_k_refill=False, first_releaser=False, early_release=False, straddle=True, break_zero=False,
+           stages=DQ_STAGES):
+    """attn_bwd_dq_wgmma_kernel: the forward's ring (`stages` deep) with Q and dO resident; S / dP read K and V and are waited for,
     V is released, then dQ += dS K reads K, is waited for, and K is released.  With `straddle` the last key tile crosses the
     sequence end, and all warps zero its K rows past the end and meet at a named barrier first.  Seeded breaks (each must be
     caught):
@@ -95,7 +96,7 @@ def run_dq(T, seed, break_k_refill=False, first_releaser=False, early_release=Fa
                       the load may land while another warp's dQ MMA still reads K;
       first_releaser  the first warp to release a stage refills it;
       early_release   K is released before the wait of the dQ MMAs that read it."""
-    NST = DQ_STAGES
+    NST = stages
     refill_at = 1 if first_releaser else WARPS
     rnd = random.Random(seed)
     B = {"qd": Bar(1), "zb": Bar(WARPS)}
