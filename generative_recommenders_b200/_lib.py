@@ -14,10 +14,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HSTU_B200_LIB") or os.path.join(_HERE, "lib", "libhstu_b200.so")
 
 ABI_VERSION = 1
-F32, BF16, F16 = 0, 1, 2
+F32, BF16, F16, E4M3 = 0, 1, 2, 3
 IMPL_AUTO, IMPL_GENERIC, IMPL_UMMA = 0, 1, 2
 
-_DTYPES = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16}
+_DTYPES = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16, torch.float8_e4m3fn: E4M3}
 
 
 class AttnParams(C.Structure):
@@ -42,6 +42,15 @@ class AttnParams(C.Structure):
     ]
 
 
+class Descales(C.Structure):
+    """hstu_attn_descales: per (sequence, head) fp32 scales of the fp8 forward's q, k, v (NULL = 1)."""
+    _fields_ = [
+        ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p),
+        ("q_batch_stride", C.c_int64), ("q_head_stride", C.c_int64), ("k_batch_stride", C.c_int64),
+        ("k_head_stride", C.c_int64), ("v_batch_stride", C.c_int64), ("v_head_stride", C.c_int64),
+    ]
+
+
 class SslParams(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("dtype", C.c_int32), ("N", C.c_int64), ("R", C.c_int32), ("D", C.c_int32),
@@ -62,6 +71,7 @@ _PROTOS = {
     "hstu_attn_workspace_bytes": (C.c_size_t, [C.POINTER(AttnParams), C.c_int]),
     "hstu_attn_fwd": (C.c_int, [C.POINTER(AttnParams), _vp]),
     "hstu_attn_bwd": (C.c_int, [C.POINTER(AttnParams), _vp]),
+    "hstu_attn_fwd_fp8": (C.c_int, [C.POINTER(AttnParams), C.POINTER(Descales), _vp]),
     "hstu_attn_select_impl": (C.c_int, [C.POINTER(AttnParams), C.c_int]),
     "hstu_mask_valid": (C.c_int, [_i32] * 7),
     "hstu_kv_range_for_q_rows": (C.c_int, [_i32] * 7 + [C.POINTER(_i32)] * 2),

@@ -21,7 +21,8 @@ static int validate_attn(const hstu_attn_params* p, bool bwd) {
   HSTU_CHECK_ARG(p != nullptr, "params is NULL");
   HSTU_CHECK_ARG(p->abi_version == HSTU_B200_ABI_VERSION, "ABI version mismatch: caller %d, library %d", p->abi_version,
                  HSTU_B200_ABI_VERSION);
-  HSTU_CHECK_ARG(p->dtype == HSTU_F32 || p->dtype == HSTU_BF16 || p->dtype == HSTU_F16, "bad dtype %d", p->dtype);
+  HSTU_CHECK_ARG(p->dtype == HSTU_F32 || p->dtype == HSTU_BF16 || p->dtype == HSTU_F16 || p->dtype == HSTU_E4M3, "bad dtype %d",
+                 p->dtype);
   HSTU_CHECK_ARG(p->max_seq_len > 0, "max_seq_len must be larger than 0");  // ops/hstu_attention.py:64
   HSTU_CHECK_ARG(p->batch >= 0 && p->heads > 0, "bad batch/heads");
   HSTU_CHECK_ARG(p->dqk > 0 && p->dv > 0 && p->dqk <= 256 && p->dv <= 256, "head dims must be in [1, 256] (dqk=%d, dv=%d)",
@@ -61,6 +62,18 @@ int bind_device(const void* ptr) {
 // A deterministic backward takes the same route as any other: the wgmma kernels run their atomic-free split path
 // (attn_wgmma_bwd.cu), and the generic kernels have no atomics on q / k / v.
 static int select_impl(const hstu_attn_params* p, bool bwd) {
+  if (p->dtype == HSTU_E4M3) {  // the fp8 forward: wgmma kernels only, whatever the device (hstu_attn_fwd_fp8 checks it)
+    if (bwd) {
+      set_error("fp8 (e4m3) attention has no backward: hstu_attn_fwd_fp8 is a forward-only entry");
+      return HSTU_ERR_UNSUPPORTED;
+    }
+    if (p->impl == HSTU_IMPL_GENERIC) {
+      set_error("fp8 (e4m3) attention runs on the wgmma kernels only: the generic kernels take no fp8 input");
+      return HSTU_ERR_UNSUPPORTED;
+    }
+    if (int e = e4m3_fwd_check(*p)) return e;
+    return HSTU_IMPL_UMMA;
+  }
   if (bwd && p->deterministic && (p->pos_w != nullptr || p->ts_w != nullptr)) {
     set_error("deterministic backward with a relative bias is not supported: the dpos_w / dts_w gradients are added "
               "with atomics");
@@ -77,6 +90,40 @@ static int select_impl(const hstu_attn_params* p, bool bwd) {
     return HSTU_IMPL_UMMA;
   }
   return can ? HSTU_IMPL_UMMA : HSTU_IMPL_GENERIC;
+}
+
+// Nullable descales: no negative strides, fp32-aligned pointers.
+static int validate_descales(const hstu_attn_descales* d) {
+  if (d == nullptr) return 0;
+  const float* ptr[3] = {d->q, d->k, d->v};
+  const int64_t bs[3] = {d->q_batch_stride, d->k_batch_stride, d->v_batch_stride};
+  const int64_t hs[3] = {d->q_head_stride, d->k_head_stride, d->v_head_stride};
+  for (int i = 0; i < 3; ++i) {
+    const char name = "qkv"[i];
+    HSTU_CHECK_ARG(bs[i] >= 0 && hs[i] >= 0, "%c descale: negative stride (batch %lld, head %lld)", name, (long long)bs[i],
+                   (long long)hs[i]);
+    HSTU_CHECK_ARG((reinterpret_cast<uintptr_t>(ptr[i]) & 3) == 0, "%c descale: %p is not a float pointer", name, (const void*)ptr[i]);
+  }
+  return 0;
+}
+
+// Every non-null descale is device memory of the device that runs the call (the current one, after bind_device).
+static int check_descale_devices(const hstu_attn_descales* d) {
+  if (d == nullptr) return 0;
+  int dev = 0;
+  HSTU_CUDA_OK(cudaGetDevice(&dev));
+  const float* ptr[3] = {d->q, d->k, d->v};
+  for (int i = 0; i < 3; ++i) {
+    if (ptr[i] == nullptr) continue;
+    cudaPointerAttributes attr;
+    const cudaError_t e = cudaPointerGetAttributes(&attr, ptr[i]);
+    if (e != cudaSuccess || (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) || attr.device != dev) {
+      cudaGetLastError();
+      set_error("%c descale: expected device memory of CUDA device %d (got %p)", "qkv"[i], dev, (const void*)ptr[i]);
+      return HSTU_ERR_INVALID_ARGUMENT;
+    }
+  }
+  return 0;
 }
 
 }  // namespace hstu
@@ -98,12 +145,14 @@ size_t hstu_attn_workspace_bytes(const hstu_attn_params* p, int is_backward) {
   if (validate_attn(p, is_backward != 0) != 0) return 0;
   if (p->batch == 0 || p->total_rows == 0) return 0;
   int impl = select_impl(p, is_backward != 0);
+  if (p->dtype == HSTU_E4M3) return impl == HSTU_IMPL_UMMA ? e4m3_v_copy_bytes(*p) : 0;  // the fp16 copy of v
   if (impl == HSTU_IMPL_UMMA) return wgmma_workspace_bytes(*p, is_backward != 0);
   return 0;
 }
 
 int hstu_attn_fwd(const hstu_attn_params* p, void* stream) {
   if (int e = validate_attn(p, false)) return e;
+  HSTU_CHECK_ARG(p->dtype != HSTU_E4M3, "hstu_attn_fwd: fp8 (e4m3) inputs go through hstu_attn_fwd_fp8 (with their descales)");
   if (p->batch == 0 || p->total_rows == 0) return 0;  // triton_hstu_attention.py:1789-1790
   if (int e = bind_device(p->q)) return e;
   int impl = select_impl(p, false);
@@ -114,12 +163,34 @@ int hstu_attn_fwd(const hstu_attn_params* p, void* stream) {
 
 int hstu_attn_bwd(const hstu_attn_params* p, void* stream) {
   if (int e = validate_attn(p, true)) return e;
+  if (p->dtype == HSTU_E4M3) {
+    set_error("hstu_attn_bwd: fp8 (e4m3) attention has no backward (hstu_attn_fwd_fp8 is forward only)");
+    return HSTU_ERR_UNSUPPORTED;
+  }
   if (p->batch == 0 || p->total_rows == 0) return 0;
   if (int e = bind_device(p->q)) return e;
   int impl = select_impl(p, true);
   if (impl < 0) return impl;
   if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bwd(*p, (cudaStream_t)stream);
   return attn_generic_bwd(*p, (cudaStream_t)stream);
+}
+
+int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* descales, void* stream) {
+  if (int e = validate_attn(p, false)) return e;
+  HSTU_CHECK_ARG(p->dtype == HSTU_E4M3, "hstu_attn_fwd_fp8: q, k, v must be HSTU_E4M3 (got dtype %d)", p->dtype);
+  if (int e = validate_descales(descales)) return e;
+  const int impl = select_impl(p, false);
+  if (impl < 0) return impl;
+  if (p->batch == 0 || p->total_rows == 0) return 0;
+  if (int e = bind_device(p->q)) return e;
+  if (int e = check_descale_devices(descales)) return e;
+  if (!is_sm90()) {
+    set_error("hstu_attn_fwd_fp8: the fp8 kernels need an sm_90 device");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  hstu_attn_descales none;
+  memset(&none, 0, sizeof(none));
+  return attn_wgmma_fwd_e4m3(*p, descales ? *descales : none, (cudaStream_t)stream);
 }
 
 int hstu_mask_valid(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,

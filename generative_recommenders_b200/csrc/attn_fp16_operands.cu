@@ -5,7 +5,10 @@
 // Both run one CTA per (256-row block, head, sequence) over the rows < max_seq_len of each sequence.  Rows of the copies
 // past max_seq_len are not written: the attention kernels treat them as rows past the sequence end, which never reach an
 // MMA (zero_tile_rows, DESIGN.md 2).
+// The fp8 forward (attn_wgmma_fwd_e4m3.cu) reuses the convert kernel to widen its e4m3 v to fp16, [L, H, dv]: every finite
+// e4m3 value is a normal fp16 value, so that copy is exact and needs no scale (and no amax pass).
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <string.h>
 
 #include "attn_fp16_operands.cuh"
@@ -17,7 +20,7 @@ namespace hstu {
 constexpr int kPreRows = 256, kPreThreads = 256, kPreD = 32;
 
 struct PreOperand {
-  const uint16_t* src;  // bf16 [L, H, 32] view
+  const void* src;      // bf16 [L, H, 32] view (e4m3 [L, H, d] for the fp8 forward's v)
   long long row_stride, head_stride;
   __half* dst;          // fp16 [L, H, 32], contiguous
 };
@@ -27,6 +30,7 @@ struct PreParams {
   int nops;  // 3 (q, k, v) or 4 (+ dO)
   const void* seq_offsets;
   int offsets_i64, max_seq_len, heads;
+  int d;  // columns of the e4m3 operand (the bf16 operands have kPreD)
   float alpha;
   uint32_t* amax;  // [B, H, kAmaxSlots], zeroed before the amax kernel
 };
@@ -48,7 +52,8 @@ __global__ void __launch_bounds__(kPreThreads) fp16_operands_amax_kernel(const _
     // 4 threads per row, 8 elements (16 bytes) each
     for (int c = threadIdx.x; c < rows * 4; c += kPreThreads) {
       const int r = c >> 2, part = c & 3;
-      const uint4 x = *reinterpret_cast<const uint4*>(op.src + (row0 + r0 + r) * op.row_stride + (long long)h * op.head_stride + part * 8);
+      const uint4 x = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(op.src) + (row0 + r0 + r) * op.row_stride +
+                                                      (long long)h * op.head_stride + part * 8);
       const uint32_t w[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -70,6 +75,9 @@ __global__ void __launch_bounds__(kPreThreads) fp16_operands_amax_kernel(const _
   }
 }
 
+// E4M3 = false: the scaled fp16 copies of the bf16 d = 32 operands.  E4M3 = true: the exact fp16 copy of an e4m3 operand of
+// p.d columns (no scale), [L, H, p.d]
+template <bool E4M3>
 __global__ void __launch_bounds__(kPreThreads) fp16_operands_convert_kernel(const __grid_constant__ PreParams p) {
   const int b = blockIdx.z, h = blockIdx.y;
   const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
@@ -77,24 +85,41 @@ __global__ void __launch_bounds__(kPreThreads) fp16_operands_convert_kernel(cons
   const int r0 = blockIdx.x * kPreRows;
   if (r0 >= len) return;
   const int rows = min(kPreRows, len - r0);
-  const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, p.alpha, kPreD);
-  const int exps[kAmaxSlots] = {ex.q, ex.k, ex.v, ex.o};
+  const int d = E4M3 ? p.d : kPreD, cpr = d / 8;  // columns; chunks of 8 elements per row
+  int exps[kAmaxSlots] = {0, 0, 0, 0};
+  if constexpr (!E4M3) {
+    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, p.alpha, kPreD);
+    exps[0] = ex.q, exps[1] = ex.k, exps[2] = ex.v, exps[3] = ex.o;
+  }
   for (int o = 0; o < p.nops; ++o) {
     const PreOperand& op = p.op[o];
     const int e = exps[o];
-    for (int c = threadIdx.x; c < rows * 4; c += kPreThreads) {
-      const int r = c >> 2, part = c & 3;
+    for (int c = threadIdx.x; c < rows * cpr; c += kPreThreads) {
+      const int r = c / cpr, part = c % cpr;
       const long long row = row0 + r0 + r;
-      const uint4 x = *reinterpret_cast<const uint4*>(op.src + row * op.row_stride + (long long)h * op.head_stride + part * 8);
-      const uint32_t w[4] = {x.x, x.y, x.z, x.w};
       uint32_t y[4];
+      if constexpr (E4M3) {
+        const uint2 x = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(op.src) + row * op.row_stride +
+                                                        (long long)h * op.head_stride + part * 8);
+        const uint32_t w[2] = {x.x, x.y};
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        // exact: a power-of-two scale of an 8-bit significand into fp16's range (scalbnf is exact wherever the result is)
-        const __half2 v = __floats2half2_rn(scalbnf(bf16_bits_to_float(w[i] & 0xffffu), e), scalbnf(bf16_bits_to_float(w[i] >> 16), e));
-        y[i] = *reinterpret_cast<const uint32_t*>(&v);
+        for (int i = 0; i < 4; ++i) {
+          // exact: e4m3 -> fp16 (NaN stays NaN)
+          const __half2_raw v = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i >> 1] >> (16 * (i & 1))), __NV_E4M3);
+          y[i] = (uint32_t)v.x | ((uint32_t)v.y << 16);
+        }
+      } else {
+        const uint4 x = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(op.src) + row * op.row_stride +
+                                                        (long long)h * op.head_stride + part * 8);
+        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          // exact: a power-of-two scale of an 8-bit significand into fp16's range (scalbnf is exact wherever the result is)
+          const __half2 v = __floats2half2_rn(scalbnf(bf16_bits_to_float(w[i] & 0xffffu), e), scalbnf(bf16_bits_to_float(w[i] >> 16), e));
+          y[i] = *reinterpret_cast<const uint32_t*>(&v);
+        }
       }
-      *reinterpret_cast<uint4*>(op.dst + (row * p.heads + h) * kPreD + part * 8) = make_uint4(y[0], y[1], y[2], y[3]);
+      *reinterpret_cast<uint4*>(op.dst + (row * p.heads + h) * d + part * 8) = make_uint4(y[0], y[1], y[2], y[3]);
     }
   }
 }
@@ -127,7 +152,7 @@ int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out
   const long long hs[kAmaxSlots] = {p.q_head_stride, p.k_head_stride, p.v_head_stride, p.do_head_stride};
   pp.nops = bwd ? 4 : 3;
   for (int o = 0; o < pp.nops; ++o) {
-    pp.op[o].src = reinterpret_cast<const uint16_t*>(src[o]);
+    pp.op[o].src = src[o];
     pp.op[o].row_stride = rs[o];
     pp.op[o].head_stride = hs[o];
     pp.op[o].dst = reinterpret_cast<__half*>(ws + align256(amax_bytes) + o * copy);
@@ -144,7 +169,35 @@ int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out
   const dim3 grid((p.max_seq_len + kPreRows - 1) / kPreRows, p.heads, p.batch);
   fp16_operands_amax_kernel<<<grid, kPreThreads, 0, st>>>(pp);
   HSTU_CUDA_OK(cudaGetLastError());
-  fp16_operands_convert_kernel<<<grid, kPreThreads, 0, st>>>(pp);
+  fp16_operands_convert_kernel<false><<<grid, kPreThreads, 0, st>>>(pp);
+  HSTU_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+size_t e4m3_v_copy_bytes(const hstu_attn_params& p) { return align256((size_t)p.total_rows * p.heads * p.dv * sizeof(__half)); }
+
+int e4m3_v_prepass(const hstu_attn_params& p, const void** v16, cudaStream_t st) {
+  const size_t need = e4m3_v_copy_bytes(p);
+  if (p.workspace == nullptr || p.workspace_bytes < need) {
+    set_error("hstu_attn_fwd_fp8: workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
+    return HSTU_ERR_WORKSPACE;
+  }
+  PreParams pp;
+  memset(&pp, 0, sizeof(pp));
+  pp.nops = 1;
+  pp.op[0].src = p.v;
+  pp.op[0].row_stride = p.v_row_stride;
+  pp.op[0].head_stride = p.v_head_stride;
+  pp.op[0].dst = reinterpret_cast<__half*>(p.workspace);
+  *v16 = p.workspace;
+  pp.seq_offsets = p.seq_offsets;
+  pp.offsets_i64 = p.offsets_are_i64;
+  pp.max_seq_len = p.max_seq_len;
+  pp.heads = p.heads;
+  pp.d = p.dv;
+  if (p.batch == 0 || p.max_seq_len <= 0) return 0;
+  const dim3 grid((p.max_seq_len + kPreRows - 1) / kPreRows, p.heads, p.batch);
+  fp16_operands_convert_kernel<true><<<grid, kPreThreads, 0, st>>>(pp);
   HSTU_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -69,6 +69,28 @@ __host__ __device__ inline OperandExps operand_exps(const uint32_t* amax, float 
   return x;
 }
 
+// Exponent p of the fp8 forward's fp16 P operand P' = P 2^p (attn_wgmma_fwd_e4m3.cu, DESIGN.md 3.5).  With e4m3 q, k
+// (|x| <= 448) and |silu y| <= |y|, |P| <= B = |alpha q_descale k_descale| d 448^2.  Writing each factor as m 2^e with m in
+// [0.5, 1) (frexp) and d <= 2^ld: B < 2^(e_a + e_q + e_k + ld + 18), so p = -3 - (e_a + e_q + e_k + ld) puts B 2^p below
+// 2^15, and (d a power of two) at or above 448^2 2^-6 > 2^11: no fp16 overflow, and no amax pass over q and k.  A zero, Inf
+// or NaN factor gives p = 0, and p is clamped to fp32's normal exponents (pow2f), as in operand_exps.
+__host__ __device__ inline int e4m3_p_exp(float alpha, float q_descale, float k_descale, int d) {
+  const float f[3] = {alpha, q_descale, k_descale};
+  int sum = 0;
+  for (int i = 0; i < 3; ++i) {
+    const float a = f[i] < 0.f ? -f[i] : f[i];
+    uint32_t bits;
+    memcpy(&bits, &a, 4);
+    bool special;
+    const int l = amax_log2(bits, &special);  // floor(log2 a) = frexp exponent - 1
+    if (special) return 0;
+    sum += l + 1;
+  }
+  int ld = 0;
+  while ((1 << ld) < d) ++ld;  // ceil(log2 d)
+  return clamp_exp(-3 - (sum + ld));
+}
+
 // 2^e for e in [-126, 127] (exact, built from the exponent bits)
 __host__ __device__ inline float pow2f(int e) {
   const uint32_t b = (uint32_t)(clamp_exp(e) + 127) << 23;

@@ -25,6 +25,15 @@ struct Fp16Operands {
 };
 size_t fp16_operands_workspace_bytes(const hstu_attn_params& p, bool bwd);
 int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out, cudaStream_t st);
+// the fp8 forward's fp16 copy of the e4m3 v, [L, H, dv] contiguous (exact: no scale), at the start of the workspace
+size_t e4m3_v_copy_bytes(const hstu_attn_params& p);
+int e4m3_v_prepass(const hstu_attn_params& p, const void** v16, cudaStream_t st);
+
+// attn_wgmma_fwd_e4m3.cu: the fp8 forward.  e4m3_fwd_check: 0 if the wgmma fp8 kernels take the shape (sizes, flags and
+// alignment only, no device query), else HSTU_ERR_UNSUPPORTED with a message
+int e4m3_fwd_check(const hstu_attn_params& p);
+int attn_wgmma_fwd_e4m3(const hstu_attn_params& p, const hstu_attn_descales& ds, cudaStream_t st);
+bool is_sm90();
 
 // norm.cu
 int layer_norm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, long long n, int D,

@@ -223,9 +223,10 @@ __device__ __forceinline__ uint32_t swizzled_chunk_offset(uint32_t row, uint32_t
 // ---------------------------------------------------------------------------------------------
 // host: tensor maps
 // ---------------------------------------------------------------------------------------------
-// 3-D map over a [rows, heads, d] bf16/fp16 tensor with arbitrary row / head strides (elements): dims (d, heads, rows),
-// box (box_cols, 1, box_rows), swizzle = box_cols * 2 bytes (32/64/128).  Returns 0 on success.
+// 3-D map over a [rows, heads, d] tensor of elem_bytes-byte elements (2: bf16 / fp16, 1: e4m3) with arbitrary row / head
+// strides (elements): dims (d, heads, rows), box (box_cols, 1, box_rows), swizzle = box_cols * elem_bytes bytes (32/64/128).
+// Returns 0 on success.
 int make_tmap_rows_heads(CUtensorMap* out, const void* base, long long rows, int heads, int d, long long row_stride,
-                         long long head_stride, int box_cols, int box_rows);
+                         long long head_stride, int box_cols, int box_rows, int elem_bytes = 2);
 
 }  // namespace hstu

@@ -4,8 +4,9 @@
 //   S = A B^T   wgmma with both operands K-major in shared memory          (score GEMMs of both kernels)
 //   O = S V     wgmma with A = S from registers (hi + lo bf16), B MN-major   (P V, dV, dK)
 //   E = W V     wgmma with A MN-major written by threads through swizzled_chunk_offset, B MN-major   (dQ = dS K)
-// Inputs are multiples of 1/8 in [-1, 1]: every product and sum is exact in fp32 (and S fits the 16 bits of hi + lo), so
-// the device results must equal the host reference exactly.
+//   S = A B^T   on e4m3 operands (m64n64k32, both K-major, byte TMA with 32B / 64B / 128B swizzle)  (scores of the fp8 forward)
+// Inputs are multiples of 1/8 in [-1, 1] (of 1/4 for e4m3): every product and sum is exact in fp32 (and S fits the 16 bits of
+// hi + lo), so the device results must equal the host reference exactly.
 #include <stdarg.h>
 #include <string.h>
 
@@ -110,6 +111,45 @@ __global__ void __launch_bounds__(128) selftest_kernel(const __grid_constant__ C
   }
 }
 
+// one warpgroup; A, B: [64 rows][D] e4m3 loaded by TMA as bytes (swizzle D bytes, D <= 128)
+template <int D>
+__global__ void __launch_bounds__(128) selftest_e4m3_kernel(const __grid_constant__ CUtensorMap tA, const __grid_constant__ CUtensorMap tB,
+                                                            float* S) {
+  constexpr int SW = D, TILE = 64 * D;
+  extern __shared__ uint8_t raw[];
+  uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
+  uint8_t *sA = sm, *sB = sm + TILE;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + 2 * TILE);
+  const int tid = threadIdx.x, w = tid >> 5, g = (tid & 31) >> 2, t4 = tid & 3;
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(bar, 2 * TILE);
+    tma_load_3d(sA, &tA, bar, 0, 0, 0);
+    tma_load_3d(sB, &tB, bar, 0, 0, 0);
+  }
+  mbar_wait(bar, 0);
+  float s[32];
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < D / 32; ++ks)
+    wgmma_ss_64_e4m3(s, desc_kmajor<SW>(smem_u32(sA), ks * 32), desc_kmajor<SW>(smem_u32(sB), ks * 32), ks > 0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(s);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = w * 16 + g + 8 * h;
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) S[row * 64 + nb * 8 + 2 * t4 + c] = s[nb * 4 + h * 2 + c];
+  }
+}
+
 static void appendf(std::string& s, const char* fmt, ...) {
   char buf[512];
   va_list ap;
@@ -197,6 +237,52 @@ static int run_case(std::string& rep) {
   return fails;
 }
 
+template <int D>
+static int run_case_e4m3(std::string& rep) {
+  constexpr int SMEM = 2 * 64 * D + 64 + 1024;
+  uint32_t rng = 777u + D;
+  // e4m3 bytes of j / 4, j in [-4, 4]: 0.25 = 2^-2 (exponent field 5), 0.5 (6), 0.75 = 1.5 * 2^-1 (6, mantissa 4), 1 (7)
+  static const uint8_t kMag[5] = {0x00, 0x28, 0x30, 0x34, 0x38};
+  std::vector<float> A(64 * D), B(64 * D);
+  std::vector<uint8_t> hA(64 * D), hB(64 * D);
+  for (int m = 0; m < 2; ++m)
+    for (int i = 0; i < 64 * D; ++i) {
+      rng = rng * 1664525u + 1013904223u;
+      const int j = (int)((rng >> 16) % 9) - 4;
+      (m ? B : A)[i] = j / 4.0f;
+      (m ? hB : hA)[i] = (uint8_t)(kMag[j < 0 ? -j : j] | (j < 0 ? 0x80 : 0));
+    }
+  std::vector<double> rS(64 * 64, 0.0);
+  for (int m = 0; m < 64; ++m)
+    for (int n = 0; n < 64; ++n)
+      for (int k = 0; k < D; ++k) rS[m * 64 + n] += (double)A[m * D + k] * B[n * D + k];
+  uint8_t *dA, *dB;
+  float* dS;
+  ST_CUDA(cudaMalloc(&dA, 64 * D));
+  ST_CUDA(cudaMalloc(&dB, 64 * D));
+  ST_CUDA(cudaMalloc(&dS, 64 * 64 * 4));
+  ST_CUDA(cudaMemcpy(dA, hA.data(), 64 * D, cudaMemcpyHostToDevice));
+  ST_CUDA(cudaMemcpy(dB, hB.data(), 64 * D, cudaMemcpyHostToDevice));
+  CUtensorMap tA, tB;
+  if (make_tmap_rows_heads(&tA, dA, 64, 1, D, D, D, D, 64, 1) || make_tmap_rows_heads(&tB, dB, 64, 1, D, D, D, D, 64, 1)) {
+    appendf(rep, "tensor map: %s\n", g_selftest_err);
+    return -1;
+  }
+  ST_CUDA(cudaFuncSetAttribute(selftest_e4m3_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  selftest_e4m3_kernel<D><<<1, 128, SMEM>>>(tA, tB, dS);
+  ST_CUDA(cudaGetLastError());
+  ST_CUDA(cudaDeviceSynchronize());
+  std::vector<float> S(64 * 64);
+  ST_CUDA(cudaMemcpy(S.data(), dS, S.size() * 4, cudaMemcpyDeviceToHost));
+  for (void* p : {(void*)dA, (void*)dB, (void*)dS}) cudaFree(p);
+  double worst = 0.0;
+  for (size_t i = 0; i < rS.size(); ++i) worst = fmax(worst, fabs((double)S[i] - rS[i]));
+  const bool ok = worst == 0.0;
+  appendf(rep, "S = A B^T  (SS, e4m3 m64n64k32, K-major x K-major) d=%d (swizzle %dB): max |device - host| = %g %s\n", D, D, worst,
+          ok ? "ok" : "FAIL");
+  return ok ? 0 : 1;
+}
+
 }  // namespace hstu
 
 extern "C" {
@@ -214,7 +300,9 @@ int hstu_umma_selftest(char* report, size_t report_bytes) {
   }
   hstu::appendf(rep, "device: %s\n", prop.name);
   int fails = 0;
-  for (int r : {hstu::run_case<32>(rep), hstu::run_case<64>(rep)}) fails = (r < 0 || fails < 0) ? -1 : fails + r;
+  for (int r : {hstu::run_case<32>(rep), hstu::run_case<64>(rep), hstu::run_case_e4m3<32>(rep), hstu::run_case_e4m3<64>(rep),
+                hstu::run_case_e4m3<128>(rep)})
+    fails = (r < 0 || fails < 0) ? -1 : fails + r;
   if (report && report_bytes) snprintf(report, report_bytes, "%s", rep.c_str());
   return fails;
 }

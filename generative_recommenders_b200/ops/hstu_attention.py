@@ -65,7 +65,15 @@ def cuda_hstu_attention_fwd(
     num_targets: Optional[torch.Tensor] = None, max_attn_len: int = 0, contextual_seq_len: int = 0,
     min_full_attn_seq_len: int = 0, impl: int = _lib.IMPL_AUTO, delta_q_len: int = 0,
     out: Optional[torch.Tensor] = None, bias: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
+    descales: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor], Optional[torch.Tensor]]] = None,
 ) -> torch.Tensor:
+    """descales: (q_descale, k_descale, v_descale) of fp8 inputs -- see cuda_hstu_attention_fwd_fp8.  q, k, v of dtype
+    torch.float8_e4m3fn take that path with or without descales."""
+    if descales is not None or any(t.dtype == _FP8 for t in (q, k, v)):
+        if bias is not None or delta_q_len:
+            raise RuntimeError("fp8 attention: the relative bias and delta_q are not supported")
+        return cuda_hstu_attention_fwd_fp8(max_seq_len, alpha, q, k, v, seq_offsets, descales, num_targets, max_attn_len,
+                                           contextual_seq_len, min_full_attn_seq_len, impl, out)
     dev = _lib.require_cuda(q, k, v, seq_offsets, num_targets)
     q, k, v = _prep(q, k, v)
     seq_offsets = seq_offsets.contiguous()
@@ -85,6 +93,57 @@ def cuda_hstu_attention_fwd(
     # bf16 at d = 32: amax and convert kernels before the attention kernel (the forward's only workspace: the fp16 copies)
     _lib.note_launch(3 if ws is not None else 1)
     del ws, keep
+    return out
+
+
+_FP8 = torch.float8_e4m3fn
+
+
+def cuda_hstu_attention_fwd_fp8(
+    max_seq_len: int, alpha: float, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, seq_offsets: torch.Tensor,
+    descales: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor], Optional[torch.Tensor]]] = None,
+    num_targets: Optional[torch.Tensor] = None, max_attn_len: int = 0, contextual_seq_len: int = 0,
+    min_full_attn_seq_len: int = 0, impl: int = _lib.IMPL_AUTO, out: Optional[torch.Tensor] = None,
+) -> torch.Tensor:
+    """Forward of attention on float8_e4m3fn q, k, v (`hstu_attn_fwd_fp8`): the bf16 result of the attention of
+    q * q_descale[b, h], k * k_descale[b, h] and v * v_descale[b, h], every mask option of the bf16 path included.  Each
+    descale is an fp32 [B, H] tensor (any strides) or None for 1.  There is no fp8 backward.  The wgmma kernels take
+    dqk == dv in {32, 64, 128, 256}, 16-byte aligned views with row / head strides that are multiples of 16 elements."""
+    if not all(t.dtype == _FP8 for t in (q, k, v)):
+        raise RuntimeError(f"fp8 attention: q, k and v must all be torch.float8_e4m3fn (got {q.dtype}, {k.dtype}, {v.dtype}); "
+                           "descales apply to fp8 inputs only")
+    dev = _lib.require_cuda(q, k, v, seq_offsets, num_targets)
+    q, k, v = _prep(q, k, v)
+    seq_offsets = seq_offsets.contiguous()
+    if num_targets is not None:
+        num_targets = num_targets.contiguous()
+    B, H = seq_offsets.numel() - 1, q.shape[1]
+    ds = _lib.Descales()
+    for name, d in zip("qkv", descales if descales is not None else (None, None, None)):
+        if d is None:
+            continue
+        if d.dtype != torch.float32 or tuple(d.shape) != (B, H):
+            raise RuntimeError(f"fp8 attention: {name}_descale must be an fp32 [B, H] = [{B}, {H}] tensor "
+                               f"(got {d.dtype} {tuple(d.shape)})")
+        if d.device != dev:
+            raise RuntimeError(f"fp8 attention: {name}_descale is on {d.device}, the inputs on {dev}")
+        setattr(ds, name, d.data_ptr())
+        setattr(ds, f"{name}_batch_stride", d.stride(0))
+        setattr(ds, f"{name}_head_stride", d.stride(1))
+    if out is None:
+        out = torch.empty((q.shape[0], H, v.shape[2]), dtype=torch.bfloat16, device=dev)
+    elif out.dtype != torch.bfloat16:
+        raise RuntimeError(f"fp8 attention: out must be bf16 (got {out.dtype})")
+    p = _lib.AttnParams()
+    _fill_common(p, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
+                 min_full_attn_seq_len, impl)
+    p.out = out.data_ptr()
+    p.o_row_stride, p.o_head_stride = out.stride(0), out.stride(1)
+    ws = _workspace(p, False, dev)
+    with torch.cuda.device(dev), _lib.timed("attn_fwd_fp8", dev):
+        _lib.check(_lib.lib().hstu_attn_fwd_fp8(C.byref(p), C.byref(ds), _lib.stream_ptr(dev)), "hstu_attn_fwd_fp8")
+    _lib.note_launch(2)  # the fp16 copy of v, then the attention kernel
+    del ws
     return out
 
 

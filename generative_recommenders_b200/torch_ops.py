@@ -6,7 +6,12 @@ implemented there for sm80 / sm90.  `register()` defines the same schemas (as a 
 already-loaded reference extension only if that one is absent -- a second definition of the same operator is an error) and
 routes them to libhstu_b200.so, so code written against `torch.ops.hstu.hstu_mha(...)` runs on H100 unchanged.
 
-Arguments this backend does not implement raise instead of being ignored: `attn_scale`, `q/k/v_descale` (fp8 paths).
+Arguments this backend does not implement raise instead of being ignored: `attn_scale` and the dense layout
+(`seq_offsets=None`).
+fp8: with q, k and v of dtype float8_e4m3fn, `hstu_mha_fwd` and `hstu_mha` run the fp8 forward (`hstu_attn_fwd_fp8`) and
+return bf16: the attention of q * q_descale[b, h], k * k_descale[b, h], v * v_descale[b, h], each descale an fp32 [B, H]
+tensor or None for 1, as in the reference's e4m3 forward.  There is no fp8 backward: `hstu_mha` raises when a gradient is
+requested through fp8 inputs.  Descales with bf16 / fp16 inputs raise.
 `deterministic=True` (or `torch.use_deterministic_algorithms(True)`) makes the backward bitwise reproducible: the wgmma
 backward then runs its atomic-free dK / dV and dQ kernels, and shapes it does not cover run the generic kernels, which have
 no atomics either.  Otherwise the wgmma backward at d = 64 / 128 accumulates dQ with fp32 atomic adds whose order varies
@@ -32,19 +37,26 @@ _BWD = ("hstu_mha_bwd(int max_seq_len, float alpha, Tensor dout, Tensor q, Tenso
         "int contextual_seq_len, bool sort_by_length, bool deterministic, int sm_margin) -> Tensor[]")
 
 
-def _check(causal, seq_offsets, attn_scale, descales):
+_FP8 = torch.float8_e4m3fn
+
+
+def _check(causal, seq_offsets, attn_scale, descales, qkv=()):
     torch._assert(causal, "only support causal attention")
     if seq_offsets is None:
         raise RuntimeError("hstu::hstu_mha on H100: the dense (seq_offsets=None) layout is not implemented; pass jagged tensors")
-    if attn_scale is not None or any(d is not None for d in descales):
-        raise RuntimeError("hstu::hstu_mha on H100: attn_scale / q,k,v_descale (fp8) are not implemented")
+    if attn_scale is not None:
+        raise RuntimeError("hstu::hstu_mha on H100: attn_scale is not implemented")
+    if any(d is not None for d in descales) and not (qkv and all(t.dtype == _FP8 for t in qkv)):
+        raise RuntimeError("hstu::hstu_mha on H100: q,k,v_descale apply to float8_e4m3fn q, k and v only "
+                           f"(got {', '.join(str(t.dtype) for t in qkv) or 'no inputs'})")
 
 
 def _fwd(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_scale, max_attn_len, min_full_attn_seq_len,
          contextual_seq_len, q_descale, k_descale, v_descale, sm_margin):
-    _check(causal, seq_offsets, attn_scale, (q_descale, k_descale, v_descale))
+    descales = (q_descale, k_descale, v_descale)
+    _check(causal, seq_offsets, attn_scale, descales, (q, k, v))
     return cuda_hstu_attention_fwd(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
-                                   min_full_attn_seq_len)
+                                   min_full_attn_seq_len, descales=descales if any(t.dtype == _FP8 for t in (q, k, v)) else None)
 
 
 def _bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, causal, num_targets, attn_scale, max_attn_len,
@@ -80,13 +92,21 @@ class _Mha(torch.autograd.Function):
 
 def _mha(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_scale, max_attn_len, min_full_attn_seq_len,
          contextual_seq_len, q_descale, k_descale, v_descale, sort_by_length, deterministic, sm_margin):
-    _check(causal, seq_offsets, attn_scale, (q_descale, k_descale, v_descale))
+    descales = (q_descale, k_descale, v_descale)
+    _check(causal, seq_offsets, attn_scale, descales, (q, k, v))
+    if any(t.dtype == _FP8 for t in (q, k, v)):
+        if torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v)):
+            raise RuntimeError("hstu::hstu_mha on H100: fp8 attention is forward only (the reference has no fp8 backward); "
+                               "run it under torch.no_grad() or on tensors that do not require grad")
+        return cuda_hstu_attention_fwd(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
+                                       contextual_seq_len, min_full_attn_seq_len, descales=descales)
     return _Mha.apply(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len, min_full_attn_seq_len,
                       contextual_seq_len, bool(deterministic))
 
 
 def _fwd_meta(max_seq_len, alpha, q, k, v, *args):
-    return q.new_empty((q.shape[0], q.shape[1], v.shape[2]), dtype=v.dtype)
+    dt = torch.bfloat16 if v.dtype == _FP8 else v.dtype  # the fp8 forward writes bf16
+    return q.new_empty((q.shape[0], q.shape[1], v.shape[2]), dtype=dt)
 
 
 def register() -> None:

@@ -45,7 +45,8 @@ extern "C" {
 
 #define HSTU_B200_ABI_VERSION 1
 
-typedef enum hstu_dtype { HSTU_F32 = 0, HSTU_BF16 = 1, HSTU_F16 = 2 } hstu_dtype;
+/* HSTU_E4M3: float8 e4m3fn q, k, v of hstu_attn_fwd_fp8 only (its output is bf16); every other entry point rejects it. */
+typedef enum hstu_dtype { HSTU_F32 = 0, HSTU_BF16 = 1, HSTU_F16 = 2, HSTU_E4M3 = 3 } hstu_dtype;
 
 typedef enum hstu_status {
   HSTU_OK = 0,
@@ -68,7 +69,7 @@ typedef enum hstu_attn_impl {
  * [seq_offsets[b], seq_offsets[b+1]).  Semantics: pt_hstu_attention.py:130-171 (see DESIGN.md).          */
 typedef struct hstu_attn_params {
   int32_t abi_version;  /* = HSTU_B200_ABI_VERSION */
-  int32_t dtype;        /* hstu_dtype of q,k,v,out,dout,dq,dk,dv */
+  int32_t dtype;        /* hstu_dtype of q,k,v,out,dout,dq,dk,dv (HSTU_E4M3: of q,k,v; out is bf16) */
   int32_t impl;         /* hstu_attn_impl */
   int32_t batch;        /* B */
   int32_t heads;        /* H */
@@ -121,12 +122,33 @@ int hstu_abi_version(void);
 
 /* Bytes of scratch the call needs (is_backward: 0 fwd, 1 bwd).  Depends only on sizes/dtype/impl/deterministic. */
 size_t hstu_attn_workspace_bytes(const hstu_attn_params* p, int is_backward);
+/* bf16 / fp16 / fp32 attention; HSTU_E4M3 inputs go through hstu_attn_fwd_fp8 (and have no backward). */
 int hstu_attn_fwd(const hstu_attn_params* p, void* cuda_stream);
 int hstu_attn_bwd(const hstu_attn_params* p, void* cuda_stream);
+
+/* Per (sequence, head) dequantisation scales of the fp8 forward.  Each pointer is an fp32 device array read at
+ * [b * batch_stride + h * head_stride] (strides in elements, >= 0), or NULL for a scale of 1. */
+typedef struct hstu_attn_descales {
+  const float* q;
+  const float* k;
+  const float* v;
+  int64_t q_batch_stride, q_head_stride;
+  int64_t k_batch_stride, k_head_stride;
+  int64_t v_batch_stride, v_head_stride;
+} hstu_attn_descales;
+/* Forward of fp8 attention (the reference's e4m3 forward, flash_api.cpp hstu_mha_fwd with q/k/v_descale): p->dtype is
+ * HSTU_E4M3 and out is bf16; out = attention(q * q_descale[b, h], k * k_descale[b, h], v * v_descale[b, h]) with every
+ * mask option of hstu_attn_fwd.  wgmma kernels only (sm_90): dqk == dv in {32, 64, 128, 256}, no delta_q, no relative
+ * bias; q / k / v bases 16-byte aligned with row and head strides that are multiples of 16 elements.  Other shapes
+ * return HSTU_ERR_UNSUPPORTED.  Needs a workspace of hstu_attn_workspace_bytes(p, 0) bytes (an fp16 copy of v).
+ * descales may be NULL (all scales 1). */
+int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* descales, void* cuda_stream);
 /* Which implementation a call would dispatch to: returns HSTU_IMPL_GENERIC or HSTU_IMPL_UMMA (<0 on error).  A
  * deterministic backward returns HSTU_IMPL_UMMA where the wgmma backward supports the shape (it then runs its atomic-free
  * dK / dV and dQ kernels), else HSTU_IMPL_GENERIC; HSTU_ERR_UNSUPPORTED with a relative bias, or with impl forced to
- * HSTU_IMPL_UMMA on a shape the wgmma backward does not support. */
+ * HSTU_IMPL_UMMA on a shape the wgmma backward does not support.  For HSTU_E4M3 the answer depends on the shape only (the
+ * workspace size must be computable without a device): HSTU_IMPL_UMMA where the fp8 forward takes the shape, whatever the
+ * device, and hstu_attn_fwd_fp8 itself then returns HSTU_ERR_UNSUPPORTED on a device other than sm_90. */
 int hstu_attn_select_impl(const hstu_attn_params* p, int is_backward);
 
 /* ---- host-side helpers (pure CPU; used by the no-GPU tests to pin the mask / tile-skipping logic) ---- */
