@@ -727,6 +727,7 @@ static bool split_dq(const hstu_attn_params& p) { return p.dqk == 32 || p.determ
 static bool fp16_copies(const hstu_attn_params& p) { return p.dtype == HSTU_BF16 && p.dqk == 32; }
 
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd) {
+  if (!bwd && p.delta_q_len > 0) return wgmma_delta_workspace_bytes(p);  // the fp32 partials of split key chunks, or 0
   if (fp16_copies(p)) return fp16_operands_workspace_bytes(p, bwd);
   if (!bwd || split_dq(p)) return 0;
   return (size_t)p.total_rows * p.heads * p.dqk * sizeof(float);  // fp32 dQ accumulator [L, H, D]

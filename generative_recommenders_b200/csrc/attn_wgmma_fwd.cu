@@ -21,9 +21,20 @@
 // the sequence end are not written).  Rows past the sequence end that a TMA box drags in are masked out of P, and zeroed in the
 // V stage of the one key tile that crosses the end (zero_tile_rows), since P = 0 does not neutralise a NaN or Inf in V.
 //
-// Reference semantics: ops/pytorch/pt_hstu_attention.py:130-171; tile skipping mirrors the idea of
+// Delta-q (kDelta, KV-cached inference, DESIGN.md 3.6): query row i of sequence b is row b * delta + i of q / out, at sequence
+// position len - delta + i; keys are the whole (unclipped) sequence; no zero-fill past max_seq_len.  The grid is (sequence x
+// head, query tile, key chunk): HSTU has no softmax, so outputs over disjoint key ranges simply add.  Each CTA takes chunk c
+// of the key tiles its rows attend (an even split in whole 64-key tiles).  With one chunk it writes out itself; with more it
+// writes unscaled fp32 partials to the workspace and delta_reduce_kernel sums them in chunk order (bitwise reproducible).
+// Padding rows past delta cost nothing: a warpgroup with no valid row issues no MMA and only releases its stages once
+// they have landed (so its releases never run ahead into the next use of a stage), and a warp with no valid row skips the
+// elementwise stage with P = 0.  bf16 keeps the hi / lo split of P at every d, d = 32 included (no pre-pass over the cache).
+//
+// Reference semantics: ops/pytorch/pt_hstu_attention.py:130-171 (delta: :175-235); tile skipping mirrors the idea of
 // ops/triton/triton_hstu_attention.py:517-543 (loop bounds from the mask) but is derived from common.cuh's ranges.
 #include <string.h>
+
+#include <algorithm>
 
 #include "attn_fp16_operands.cuh"
 #include "common.cuh"
@@ -46,6 +57,9 @@ struct alignas(64) FwdParams {
   float inv_n;       // 1 / max_seq_len
   const uint32_t* amax;  // fp16 kernel on scaled copies of bf16 inputs: [B, H, 4] amax bits (attn_fp16_operands.cuh); else null
   int heads;
+  // delta-q only (kDelta): query rows per sequence, and with gridDim.z > 1 key chunks the fp32 partials [chunks, B * delta, H, D]
+  int delta;
+  float* part;
 };
 
 template <int D>
@@ -76,29 +90,60 @@ struct FwdBars {
   uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
 };
 
-template <int D, bool BF16>
-__global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_kernel(const __grid_constant__ FwdParams p) {
+// Delta-q: the output row (of q / out, and of the partials of chunk blockIdx.z) of local query row 0 of the CTA, and the CTA's
+// valid query rows.  Recomputed from the grid where needed, so that nothing extra stays live through the key loop.
+struct DeltaRows {
+  long long out_row, part_row;
+  int rows;
+};
+template <int BM>
+__device__ __forceinline__ DeltaRows delta_rows(const FwdParams& p) {
+  const int m0 = (int)blockIdx.y * BM;
+  const long long r = (long long)(blockIdx.x / p.heads) * p.delta + m0;
+  return {r, (long long)blockIdx.z * (gridDim.x / p.heads) * p.delta + r, min(BM, p.delta - m0)};
+}
+
+// kDelta: the delta-q geometry and key chunks described at the top (grid (B * H, query tiles, chunks)); otherwise the full
+// attention of grid (query tiles, H, B).  The two kernels below are its only instantiations.
+template <int D, bool BF16, bool kDelta>
+__device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
   using Cfg = FwdCfg<D>;
   constexpr int SW = Cfg::SW, BN = Cfg::BN, NST = Cfg::STAGES;
   // d <= 64: P V of tile i and S of tile i + 1 form one MMA batch with one wait (both fit in 128 registers); larger d waits
   // for each batch separately, since the O accumulator leaves no room for S next to the P fragments
   constexpr bool kMerge = D <= 64;
-  const int b = blockIdx.z, h = blockIdx.y;
-  const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
+  const int b = kDelta ? (int)blockIdx.x / p.heads : (int)blockIdx.z, h = kDelta ? (int)blockIdx.x % p.heads : (int)blockIdx.y;
+  const int m0 = kDelta ? (int)blockIdx.y * Cfg::BM : (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;  // first query row of the CTA
   const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
   int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
-  if (len > p.max_seq_len) {  // rows past max_seq_len are ignored on the way in and zero on the way out
+  if (!kDelta && len > p.max_seq_len) {  // rows past max_seq_len are ignored on the way in and zero on the way out
     if (blockIdx.x == 0) zero_rows(p.out, 2, p.o_row_stride, (long long)h * p.o_head_stride, D, row0 + p.max_seq_len, row0 + len);
     len = p.max_seq_len;
   }
-  if (m0 >= len) return;
+  if (!kDelta && m0 >= len) return;
+  const int p0 = kDelta ? len - p.delta + m0 : m0;  // sequence position of query row m0 (delta: the last delta rows)
   const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
   const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
-  const int mrows = min(Cfg::BM, len - m0);
+  const int mrows = min(Cfg::BM, (kDelta ? p.delta : len) - m0);
   int lo, hi;
-  kv_range_for_q_rows(msk, m0, m0 + mrows, &lo, &hi);
-  const int t0 = lo / BN;
-  const int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
+  kv_range_for_q_rows(msk, p0, p0 + mrows, &lo, &hi);
+  int t0 = lo / BN;
+  int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
+  if constexpr (kDelta) {
+    // chunk blockIdx.z of gridDim.z even shares of whole tiles; an empty share (or no key at all) writes zeros, so that
+    // every partial the reduction reads is defined
+    const int per = (T + (int)gridDim.z - 1) / (int)gridDim.z;
+    t0 += (int)blockIdx.z * per;
+    T = min(per, T - (int)blockIdx.z * per);
+    if (T <= 0) {
+      const DeltaRows dr = delta_rows<Cfg::BM>(p);
+      for (int idx = threadIdx.x; idx < dr.rows * D; idx += kFwdThreads) {
+        if (gridDim.z > 1) p.part[((dr.part_row + idx / D) * p.heads + h) * D + idx % D] = 0.f;
+        else reinterpret_cast<uint16_t*>(p.out)[(dr.out_row + idx / D) * p.o_row_stride + (long long)h * p.o_head_stride + idx % D] = 0;
+      }
+      return;
+    }
+  }
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -137,7 +182,8 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
     mbar_arrive_expect_tx(&bars->q_full, Cfg::Q_BYTES);
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx)
-      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
+      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::BOX_COLS, h,
+                  kDelta ? b * p.delta + m0 : (int)(row0 + m0));
     for (int i = 0; i < min(T, NST); ++i) {
       load(&p.tmK, Cfg::OFF_K, bars->k_full, i);
       load(&p.tmV, Cfg::OFF_V, bars->v_full, i);
@@ -146,13 +192,41 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
   __syncwarp();
 
   const int wgi = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
-  const int q_base = m0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
+  if constexpr (kDelta) {
+    if (wgi * 64 >= mrows) {
+      // a warpgroup of padding rows only: no MMA, no tanh, no output.  It still releases every stage use, once that use has
+      // landed (its full barrier), so that its releases cannot run ahead into the next use of the stage and complete a
+      // release while another warp still reads it; and it helps zero the V rows past the sequence end (CTA-wide barrier)
+      mbar_wait(&bars->k_full[0], 0);
+      release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, 0);
+      for (int i = 0; i < T; ++i) {
+        const int st = i % NST;
+        const bool next = i + 1 < T;
+        const int n0 = (t0 + i) * BN;
+        mbar_wait(&bars->v_full[st], (i / NST) & 1);
+        if (n0 + BN > len) {
+          zero_tile_rows<BN, SW, Cfg::NBOX, kFwdThreads>(smem + Cfg::OFF_V + st * Cfg::KV_BYTES, len - n0);
+          fence_proxy_async_smem();
+          named_bar_sync(kBarZeroRows, kFwdThreads);
+        }
+        if (next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+        __syncwarp();
+        release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i);
+        if (next) release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i + 1);
+        __syncwarp();
+      }
+      return;
+    }
+  }
+  const int q_base = p0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
+  // delta: a warp whose 16 rows all lie past delta skips the elementwise stage (warp-uniform)
+  const bool rows_idle = kDelta && wgi * 64 + w * 16 >= mrows;
   const uint32_t sq = smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW;
   const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
   const bool fast = msk.fast != 0;
-  const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
+  const int full_lim = fast ? min(p0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
   // scaled fp16 operands: S holds 2^(e_q + e_k) S, P is formed as 2^e_p P and O holds 2^(e_p + e_v) O
-  constexpr bool kScaled = !BF16 && D == 32;  // the only instantiation that runs bf16 inputs on fp16 copies
+  constexpr bool kScaled = !kDelta && !BF16 && D == 32;  // the only instantiation that runs bf16 inputs on fp16 copies
   float c_s = p.alpha_half, c_p = 1.f;
   int e_out = 0;
   if (kScaled && p.amax != nullptr) {
@@ -201,38 +275,41 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
       const float x = s[n] * c_s, xp = kScaled ? x * c_p : x;
       return __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
     };
-    if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
+    // a warp of padding rows only (delta) skips this stage: its A fragments keep the zeros they start with, so its P is 0
+    if (!rows_idle) {
+      if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
 #pragma unroll
-      for (int n = 0; n < BN / 2; ++n) s[n] = silu(n);
-    } else if (fast) {
-      // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limits of the thread's two rows hoisted
-      int lim[2];
+        for (int n = 0; n < BN / 2; ++n) s[n] = silu(n);
+      } else if (fast) {
+        // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limits of the thread's two rows hoisted
+        int lim[2];
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
+        for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
 #pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
+        for (int nb = 0; nb < BN / 8; ++nb)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float pv = silu(nb * 4 + e);
-          s[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? pv : 0.f;
-        }
-    } else {
+          for (int e = 0; e < 4; ++e) {
+            const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+            const float pv = silu(nb * 4 + e);
+            s[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? pv : 0.f;
+          }
+      } else {
 #pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
+        for (int nb = 0; nb < BN / 8; ++nb)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float pv = silu(nb * 4 + e);
-          s[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
-        }
-    }
+          for (int e = 0; e < 4; ++e) {
+            const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+            const float pv = silu(nb * 4 + e);
+            s[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
+          }
+      }
 #pragma unroll
-    for (int kk = 0; kk < BN / 16; ++kk) {
-      const Operand<BF16> x0(s[8 * kk + 0], s[8 * kk + 1]), x1(s[8 * kk + 2], s[8 * kk + 3]);
-      const Operand<BF16> x2(s[8 * kk + 4], s[8 * kk + 5]), x3(s[8 * kk + 6], s[8 * kk + 7]);
-      a_hi[kk][0] = x0.hi; a_hi[kk][1] = x1.hi; a_hi[kk][2] = x2.hi; a_hi[kk][3] = x3.hi;
-      a_lo[kk][0] = x0.lo; a_lo[kk][1] = x1.lo; a_lo[kk][2] = x2.lo; a_lo[kk][3] = x3.lo;
+      for (int kk = 0; kk < BN / 16; ++kk) {
+        const Operand<BF16> x0(s[8 * kk + 0], s[8 * kk + 1]), x1(s[8 * kk + 2], s[8 * kk + 3]);
+        const Operand<BF16> x2(s[8 * kk + 4], s[8 * kk + 5]), x3(s[8 * kk + 6], s[8 * kk + 7]);
+        a_hi[kk][0] = x0.hi; a_hi[kk][1] = x1.hi; a_hi[kk][2] = x2.hi; a_hi[kk][3] = x3.hi;
+        a_lo[kk][0] = x0.lo; a_lo[kk][1] = x1.lo; a_lo[kk][2] = x2.lo; a_lo[kk][3] = x3.lo;
+      }
     }
     mbar_wait(&bars->v_full[st], (i / NST) & 1);
     // the last tile may cross the sequence end: its V rows >= len belong to the next sequence (P is 0 there, V may be NaN)
@@ -270,6 +347,28 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
   }
 
   // ---------------- epilogue: O * 1/N -> global ----------------
+  if constexpr (kDelta) {  // row (local row lr) of out, or with more than one chunk the unscaled fp32 partial
+    const DeltaRows dr = delta_rows<Cfg::BM>(p);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int lr = wgi * 64 + w * 16 + g + hh * 8;
+      if (lr >= dr.rows) continue;
+      if (gridDim.z > 1) {
+        float* prow = p.part + ((dr.part_row + lr) * p.heads + h) * D;
+#pragma unroll
+        for (int nb = 0; nb < D / 8; ++nb)
+          *reinterpret_cast<float2*>(prow + nb * 8 + 2 * t4) = make_float2(o[nb * 4 + hh * 2], o[nb * 4 + hh * 2 + 1]);
+      } else {
+        uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (dr.out_row + lr) * p.o_row_stride + (long long)h * p.o_head_stride;
+#pragma unroll
+        for (int nb = 0; nb < D / 8; ++nb) {
+          const float a = o[nb * 4 + hh * 2] * p.inv_n, c = o[nb * 4 + hh * 2 + 1] * p.inv_n;
+          *reinterpret_cast<uint32_t*>(orow + nb * 8 + 2 * t4) = BF16 ? pack_bf16x2(a, c) : pack_f16x2(a, c);
+        }
+      }
+    }
+    return;
+  }
   const bool out_bf16 = BF16 || p.amax != nullptr;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
@@ -286,9 +385,58 @@ __global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_
   }
 }
 
+template <int D, bool BF16>
+__global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_kernel(const __grid_constant__ FwdParams p) {
+  attn_fwd_wgmma_body<D, BF16, false>(p);
+}
+template <int D, bool BF16>
+__global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_delta_wgmma_kernel(const __grid_constant__ FwdParams p) {
+  attn_fwd_wgmma_body<D, BF16, true>(p);
+}
+
+// Split delta-q: out = (sum of the chunks' fp32 partials [chunks, rows, H, d], in chunk order) * 1/N, 4 columns per thread.
+template <bool BF16>
+__global__ void __launch_bounds__(256) delta_reduce_kernel(const float* __restrict__ part, void* out, long long rows, int heads, int d,
+                                                            int chunks, long long o_row_stride, long long o_head_stride, float inv_n) {
+  const long long plane = rows * heads * d, n4 = plane / 4;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
+    float4 a = reinterpret_cast<const float4*>(part)[i];
+    for (int c = 1; c < chunks; ++c) {
+      const float4 x = reinterpret_cast<const float4*>(part + c * plane)[i];
+      a.x += x.x, a.y += x.y, a.z += x.z, a.w += x.w;
+    }
+    const long long e = i * 4, r = e / ((long long)heads * d), hc = e % ((long long)heads * d);
+    const long long off = r * o_row_stride + (hc / d) * o_head_stride + hc % d;
+    a.x *= inv_n, a.y *= inv_n, a.z *= inv_n, a.w *= inv_n;
+    const uint2 v = BF16 ? make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w)) : make_uint2(pack_f16x2(a.x, a.y), pack_f16x2(a.z, a.w));
+    *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(out) + off) = v;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------
+// Key chunks of a delta-q call, from sizes only (no device query, no read of seq_offsets).  The CTAs of one chunk are
+// B * H * ceil(delta / 128); the keys are split only while those fill fewer than kDeltaCtaTarget CTAs (two per SM of a 132-SM
+// H100), into at most kDeltaCtaTarget / CTAs chunks and at most ceil(N / kDeltaChunkKeys), so that no chunk of a full-length
+// sequence is shorter than 8 key tiles.  chunks * CTAs <= kDeltaCtaTarget bounds the workspace of the partials by
+// kDeltaCtaTarget * 128 rows * d * 4 bytes: 34.6 MB at d = 256, 4.3 MB at d = 32.
+// The sizing constants assume the 132 SMs of an H100 SXM; on another part they only shift the balance, never the result.
+constexpr int kH100Sms = 132;
+constexpr int kDeltaCtaTarget = 2 * kH100Sms, kDeltaChunkKeys = 512;
+constexpr int kDeltaReduceBlocks = 8 * kH100Sms;  // grid cap of delta_reduce_kernel (grid-strided: any grid is correct)
+static int delta_chunks(const hstu_attn_params& p) {
+  const long long ctas = (long long)p.batch * p.heads * ((p.delta_q_len + FwdCfg<32>::BM - 1) / FwdCfg<32>::BM);
+  if (ctas >= kDeltaCtaTarget) return 1;
+  const long long by_len = ((long long)p.max_seq_len + kDeltaChunkKeys - 1) / kDeltaChunkKeys;
+  return (int)std::max(1ll, std::min(by_len, kDeltaCtaTarget / ctas));
+}
+
+size_t wgmma_delta_workspace_bytes(const hstu_attn_params& p) {
+  const int c = delta_chunks(p);
+  return c > 1 ? (size_t)c * p.batch * p.delta_q_len * p.heads * p.dv * sizeof(float) : 0;
+}
+
 bool is_sm90() {
   static int cached = -1;
   if (cached < 0) {
@@ -306,20 +454,31 @@ bool aligned_view(const void* ptr, long long row_stride, long long head_stride) 
 bool wgmma_fwd_supported(const hstu_attn_params& p) {
   if (p.dtype != HSTU_BF16 && p.dtype != HSTU_F16) return false;
   if (p.dqk != p.dv || (p.dqk != 32 && p.dqk != 64 && p.dqk != 128 && p.dqk != 256)) return false;
-  if (p.delta_q_len != 0 || p.pos_w != nullptr || p.ts_w != nullptr) return false;
-  if (p.total_rows >= (1ll << 31) - 256) return false;
+  if (p.delta_q_len < 0 || p.pos_w != nullptr || p.ts_w != nullptr) return false;
+  if (p.total_rows >= (1ll << 31) - 256 || (long long)p.batch * p.delta_q_len >= (1ll << 31) - 256) return false;
   if (!aligned_view(p.q, p.q_row_stride, p.q_head_stride) || !aligned_view(p.k, p.k_row_stride, p.k_head_stride) ||
       !aligned_view(p.v, p.v_row_stride, p.v_head_stride) || !aligned_view(p.out, p.o_row_stride, p.o_head_stride))
     return false;
   return is_sm90();
 }
 
-// f16: the scaled fp16 copies of bf16 inputs (the kernel is then the fp16 one), or null
-template <int D, bool BF16>
+// f16: the scaled fp16 copies of bf16 inputs (the kernel is then the fp16 one), or null.  kDelta: a delta-q call, with the key
+// chunks of delta_chunks and, for more than one, the partials in the workspace and delta_reduce_kernel after the attention
+template <int D, bool BF16, bool kDelta = false>
 static int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp16Operands* f16 = nullptr) {
   using Cfg = FwdCfg<D>;
   FwdParams fp;
   memset(&fp, 0, sizeof(fp));
+  const int chunks = kDelta ? delta_chunks(p) : 1;
+  if (chunks > 1) {
+    const size_t need = wgmma_delta_workspace_bytes(p);
+    if (p.workspace == nullptr || p.workspace_bytes < need) {
+      set_error("hstu_attn_fwd: delta_q workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
+      return HSTU_ERR_WORKSPACE;
+    }
+    fp.part = reinterpret_cast<float*>(p.workspace);
+  }
+  const long long q_rows = kDelta ? (long long)p.batch * p.delta_q_len : p.total_rows;
   const long long crs = (long long)p.heads * D, chs = D;  // strides of the contiguous copies
   if (f16) {
     if (int e = make_tmap_rows_heads(&fp.tmQ, f16->copy[0], p.total_rows, p.heads, D, crs, chs, Cfg::BOX_COLS, Cfg::BM)) return e;
@@ -327,7 +486,7 @@ static int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp
     if (int e = make_tmap_rows_heads(&fp.tmV, f16->copy[2], p.total_rows, p.heads, D, crs, chs, Cfg::BOX_COLS, Cfg::BN)) return e;
     fp.amax = f16->amax;
   } else {
-    if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, p.total_rows, p.heads, D, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BM)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, q_rows, p.heads, D, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BM)) return e;
     if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, D, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
     if (int e = make_tmap_rows_heads(&fp.tmV, p.v, p.total_rows, p.heads, D, p.v_row_stride, p.v_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
   }
@@ -345,16 +504,36 @@ static int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp
   fp.ctx = p.contextual_seq_len;
   fp.alpha_half = 0.5f * p.alpha;
   fp.inv_n = 1.0f / (float)p.max_seq_len;
-  auto kern = attn_fwd_wgmma_kernel<D, BF16>;
+  fp.delta = p.delta_q_len;
+  auto kern = [] {
+    if constexpr (kDelta) return attn_fwd_delta_wgmma_kernel<D, BF16>;
+    else return attn_fwd_wgmma_kernel<D, BF16>;
+  }();
   HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  dim3 grid((p.max_seq_len + Cfg::BM - 1) / Cfg::BM, p.heads, p.batch);
+  const dim3 grid = kDelta ? dim3(p.batch * p.heads, (p.delta_q_len + Cfg::BM - 1) / Cfg::BM, chunks)
+                           : dim3((p.max_seq_len + Cfg::BM - 1) / Cfg::BM, p.heads, p.batch);
   kern<<<grid, kFwdThreads, Cfg::SMEM_BYTES, st>>>(fp);
   HSTU_CUDA_OK(cudaGetLastError());
+  if (chunks > 1) {
+    const long long n4 = q_rows * p.heads * D / 4;
+    const int blocks = (int)std::min<long long>((n4 + 255) / 256, kDeltaReduceBlocks);
+    delta_reduce_kernel<BF16><<<blocks, 256, 0, st>>>(fp.part, p.out, q_rows, p.heads, D, chunks, p.o_row_stride, p.o_head_stride,
+                                                      fp.inv_n);
+    HSTU_CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }
 
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st) {
   const bool bf = p.dtype == HSTU_BF16;
+  if (p.delta_q_len > 0) {  // bf16 keeps the hi / lo P at d = 32 too: a pre-pass over the whole cache would cost more than it saves
+    switch (p.dqk) {
+      case 32: return bf ? launch_fwd_wgmma<32, true, true>(p, st) : launch_fwd_wgmma<32, false, true>(p, st);
+      case 64: return bf ? launch_fwd_wgmma<64, true, true>(p, st) : launch_fwd_wgmma<64, false, true>(p, st);
+      case 128: return bf ? launch_fwd_wgmma<128, true, true>(p, st) : launch_fwd_wgmma<128, false, true>(p, st);
+      case 256: return bf ? launch_fwd_wgmma<256, true, true>(p, st) : launch_fwd_wgmma<256, false, true>(p, st);
+    }
+  }
   switch (p.dqk) {
     case 32: {  // bf16: the fp16 kernel on exactly scaled copies (DESIGN.md 3.0)
       if (!bf) return launch_fwd_wgmma<32, false>(p, st);

@@ -17,6 +17,8 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd);
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
+// the delta-q forward's fp32 partials of its key chunks (0 when one chunk suffices); sizes only
+size_t wgmma_delta_workspace_bytes(const hstu_attn_params& p);
 
 // attn_fp16_operands.cu: per (sequence, head) amax and exactly scaled fp16 copies of the bf16 d = 32 operands
 struct Fp16Operands {

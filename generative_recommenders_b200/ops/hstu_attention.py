@@ -90,8 +90,10 @@ def cuda_hstu_attention_fwd(
     ws = _workspace(p, False, dev)
     with torch.cuda.device(dev), _lib.timed("attn_fwd", dev):
         _lib.check(_lib.lib().hstu_attn_fwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_fwd")
-    # bf16 at d = 32: amax and convert kernels before the attention kernel (the forward's only workspace: the fp16 copies)
-    _lib.note_launch(3 if ws is not None else 1)
+    if delta_q_len:  # a workspace holds the partials of split key chunks: the attention kernel, then their reduction
+        _lib.note_launch(2 if ws is not None else 1)
+    else:  # bf16 at d = 32: amax and convert kernels before the attention kernel (the workspace: the fp16 copies)
+        _lib.note_launch(3 if ws is not None else 1)
     del ws, keep
     return out
 

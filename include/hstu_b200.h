@@ -61,7 +61,8 @@ typedef enum hstu_status {
 typedef enum hstu_attn_impl {
   HSTU_IMPL_AUTO = 0,  /* wgmma/TMA kernels when the shape allows, else the generic kernels */
   HSTU_IMPL_GENERIC = 1, /* CUDA-core fp32-accumulate kernels: any dtype / head dim <= 256 / all mask options */
-  HSTU_IMPL_UMMA = 2   /* force wgmma + TMA kernels (bf16/fp16, dqk == dv in {32, 64, 128, 256}; backward up to 128) */
+  HSTU_IMPL_UMMA = 2   /* force wgmma + TMA kernels (bf16/fp16, dqk == dv in {32, 64, 128, 256}, delta_q included;
+                          backward up to 128) */
 } hstu_attn_impl;
 
 /* One jagged attention problem: q,k [L, H, dqk], v [L, H, dv], last-dim stride 1, arbitrary row and head
@@ -81,7 +82,9 @@ typedef struct hstu_attn_params {
   int32_t max_attn_len;           /* 0 = unlimited */
   int32_t min_full_attn_seq_len;  /* only used when max_attn_len > 0 */
   int32_t contextual_seq_len;
-  int32_t delta_q_len;  /* 0 = full attention; > 0: q is [B*delta_q_len, H, dqk], the last rows of each sequence */
+  int32_t delta_q_len;  /* 0 = full attention; > 0: q is [B*delta_q_len, H, dqk], the last rows of each sequence (forward
+                           only; keys are every row of the sequence, not clipped to max_seq_len).  On the wgmma path the
+                           keys may be split into chunks whose fp32 partials need hstu_attn_workspace_bytes() of scratch */
   int32_t offsets_are_i64;      /* seq_offsets element type: 0 = int32, 1 = int64 */
   int32_t num_targets_are_i64;  /* num_targets element type */
   const void* seq_offsets;      /* [B+1] device */

@@ -82,6 +82,82 @@ def run(T, d, seed, break_refill=False, first_releaser=False, early_release=Fals
     return _eng._simulate({f"W{w}": W(w) for w in range(WARPS)}, B, rnd)
 
 
+def run_delta(T, d, seed, idle_warps=4, straddle=True, break_idle_wait=False):
+    """The delta-q variant of the forward kernel (attn_fwd_delta_wgmma_kernel): the warps of a warpgroup whose 64 query rows all
+    lie past delta (W4..W7 with idle_warps=4, none with 0) issue no MMA and read nothing; they release every K / V stage use
+    once its full barrier has completed, and take part in zeroing the V rows past the sequence end.  The other warps run the
+    forward's schedule, as in run().  Seeded break (must be caught): break_idle_wait, the idle warps release without waiting
+    for the stage to land, so their releases can run into the next use of a stage and complete it while a stage is read."""
+    NST = STAGES[d]
+    merge = d <= 64
+    rnd = random.Random(seed)
+    B = {"q": Bar(1), "zb": Bar(WARPS)}
+    R = {}
+    for i in range(NST):
+        B[f"kf{i}"], B[f"vf{i}"] = Bar(1), Bar(1)
+        R[f"k{i}"], R[f"v{i}"] = Release(), Release()
+
+    def rel(kind, i):
+        if i + NST < T:
+            st = i % NST
+            yield from release(R[f"{kind}{st}"], [("tma", f"{kind}f{st}", f"{kind}{st}")])
+
+    def active(w):
+        if w == 0:
+            yield ("async", "q")
+            for i in range(min(T, NST)):
+                yield ("tma", f"kf{i}", f"k{i}")
+                yield ("tma", f"vf{i}", f"v{i}")
+        yield ("wait", "q", 0)
+        yield ("wait", "kf0", 0)
+        yield ("read", "k0", 1)
+        yield ("read", "k0", -1)
+        yield from rel("k", 0)
+        for i in range(T):
+            st, nst = i % NST, (i + 1) % NST
+            nxt = i + 1 < T
+            yield ("wait", f"vf{st}", i // NST)
+            if straddle and not nxt:
+                yield from zero_rows(f"v{st}", "zb", 0)
+            if merge and nxt:
+                yield ("wait", f"kf{nst}", (i + 1) // NST)
+            yield ("read", f"v{st}", 1)
+            if merge and nxt:
+                yield ("read", f"k{nst}", 1)
+            yield ("read", f"v{st}", -1)
+            if merge and nxt:
+                yield ("read", f"k{nst}", -1)
+            yield from rel("v", i)
+            if not merge and nxt:
+                yield ("wait", f"kf{nst}", (i + 1) // NST)
+                yield ("read", f"k{nst}", 1)
+                yield ("read", f"k{nst}", -1)
+            if nxt:
+                yield from rel("k", i + 1)
+
+    def idle(w):  # releases without having read
+        if not break_idle_wait:
+            yield ("wait", "kf0", 0)
+        yield from rel("k", 0)
+        for i in range(T):
+            st, nst = i % NST, (i + 1) % NST
+            nxt = i + 1 < T
+            if not break_idle_wait:
+                yield ("wait", f"vf{st}", i // NST)
+            if straddle and not nxt:
+                if break_idle_wait:  # the zeroing itself still needs the landed stage
+                    yield ("wait", f"vf{st}", i // NST)
+                yield from zero_rows(f"v{st}", "zb", 0)
+            if nxt and not break_idle_wait:
+                yield ("wait", f"kf{nst}", (i + 1) // NST)
+            yield from rel("v", i)
+            if nxt:
+                yield from rel("k", i + 1)
+
+    actors = {f"W{w}": (idle(w) if w >= WARPS - idle_warps else active(w)) for w in range(WARPS)}
+    return _eng._simulate(actors, B, rnd)
+
+
 DQ_STAGES = 3  # DqCfg<D>::STAGES (csrc/attn_wgmma_bwd.cu, every d)
 
 
