@@ -657,19 +657,31 @@ def research_block_fwd(
     linear_dim: int,
     concat_ua: bool = False,
     eps: float = 1e-6,
+    store: Optional[torch.dtype] = None,
 ) -> torch.Tensor:
     """SequentialTransductionUnitJagged.forward, "rel_bias" normalisation, silu activation, no cache, dropout 0
     (research/modeling/sequential/hstu.py:318-436): LN without affine (:276-277) -> mm (no bias) -> SiLU on ALL of uvqk
     (:322-323) -> split u|v|q|k (:326-335) -> rel-bias attention (:343-357) -> u * LN(attn) or cat[u, a, u*a] with
-    a = LN(attn) (:418-422) -> Linear(+bias) + x (:424-433).  Differentiable (torch ops only)."""
+    a = LN(attn) (:418-422) -> Linear(+bias) + x (:424-433).  Differentiable (torch ops only).
+
+    store: evaluate in x.dtype but round to `store` wherever a block that keeps its activations in that dtype stores one
+    (normed x, x W, silu(x W), the attention, x + bias, the output-stage result and its product with the output weight --
+    a 16-bit addmm rounds that product before it adds the residual; the block output is left unrounded, so that its own
+    storage rounding is measured against this); the rounding is differentiable as the identity."""
     H, dqk, dv = num_heads, attention_dim, linear_dim
     dt = x.dtype
-    normed = torch.nn.functional.layer_norm(x, [x.shape[1]], eps=eps)
-    mm = torch.nn.functional.silu(torch.mm(normed, uvqk))
+
+    def rs(t):
+        return t if store is None else t.to(store).to(dt)
+
+    normed = rs(torch.nn.functional.layer_norm(x, [x.shape[1]], eps=eps))
+    mm = rs(torch.nn.functional.silu(rs(torch.mm(normed, uvqk))))
     u, v, q, k = torch.split(mm, [dv * H, dv * H, dqk * H, dqk * H], dim=1)
     L = x.shape[0]
-    attn = hstu_rel_bias_attention_fwd(n, q.reshape(L, H, dqk), k.reshape(L, H, dqk), v.reshape(L, H, dv), seq_offsets,
-                                       pos_w, ts_w, timestamps, dtype=dt).reshape(L, H * dv)
+    attn = rs(hstu_rel_bias_attention_fwd(n, q.reshape(L, H, dqk), k.reshape(L, H, dqk), v.reshape(L, H, dv), seq_offsets,
+                                          pos_w, ts_w, timestamps, dtype=dt).reshape(L, H * dv))
     a = torch.nn.functional.layer_norm(attn, [H * dv], eps=eps)
-    o_in = torch.cat([u, a, u * a], dim=-1) if concat_ua else u * a
-    return torch.nn.functional.linear(o_in, o_weight, o_bias) + x
+    o_in = rs(torch.cat([u, a, u * a], dim=-1) if concat_ua else u * a)
+    if store is None:
+        return torch.nn.functional.linear(o_in, o_weight, o_bias) + x
+    return rs(x + o_bias) + rs(o_in @ o_weight.t())
