@@ -41,6 +41,8 @@
 // kernel dQ is accumulated in fp32, not in the input dtype (triton_attention_utils.py:47-60).
 #include <string.h>
 
+#include <type_traits>
+
 #include "attn_fp16_operands.cuh"
 #include "common.cuh"
 #include "internal.h"
@@ -514,9 +516,8 @@ __global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dq_
   }
   __syncthreads();
 
-  // TMA issue of key tile i into its K or V stage (tm = &p.tmK / &p.tmV, off = Cfg::OFF_K / OFF_V, full = its full barriers)
-  auto load = [&](const CUtensorMap* tm, int off, uint64_t* full, int i) {
-    const int st = i % NST;
+  // TMA issue of key tile i into its K or V stage st (tm = &p.tmK / &p.tmV, off = Cfg::OFF_K / OFF_V, full = its full barriers)
+  auto load = [&](const CUtensorMap* tm, int off, uint64_t* full, int i, int st) {
     mbar_arrive_expect_tx(&full[st], Cfg::KV_BYTES);
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx)
@@ -526,8 +527,9 @@ __global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dq_
   // Thread 0 loads Q, dO and the first STAGES key tiles.  Afterwards each warp releases the V stage of tile i once its S / dP
   // MMAs have completed and the K stage once its dQ MMAs have, and the warp whose release is the last of the eight loads tile
   // i + STAGES into the stage (the forward's protocol).
-  auto release = [&](const CUtensorMap* tm, int off, uint64_t* full, uint32_t* ctr, int i) {
-    if (lane == 0 && i + NST < T && release_is_last<kBwdThreads / 32>(&ctr[i % NST])) load(tm, off, full, i + NST);
+  // (st: the stage of tile i, i % NST)
+  auto release = [&](const CUtensorMap* tm, int off, uint64_t* full, uint32_t* ctr, int i, int st) {
+    if (lane == 0 && i + NST < T && release_is_last<kBwdThreads / 32>(&ctr[st])) load(tm, off, full, i + NST, st);
   };
   if (tid == 0) {
     prefetch_tensormap(&p.tmQ);
@@ -541,16 +543,21 @@ __global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dq_
       tma_load_3d(smem + Cfg::OFF_DO + bx * Cfg::Q_BOX, &p.tmDO, &bars->qd_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
     }
     for (int i = 0; i < min(T, NST); ++i) {
-      load(&p.tmK, Cfg::OFF_K, bars->k_full, i);
-      load(&p.tmV, Cfg::OFF_V, bars->v_full, i);
+      load(&p.tmK, Cfg::OFF_K, bars->k_full, i, i);
+      load(&p.tmV, Cfg::OFF_V, bars->v_full, i, i);
     }
   }
   __syncwarp();
 
-  const int wgi = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
+  const int wgi = warpgroup_index(), w = warp & 3, g = lane >> 2, t4 = lane & 3;
   const int q_base = m0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
-  const uint32_t sq = smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW, sdo = smem_u32(smem + Cfg::OFF_DO) + wgi * 64 * SW;
-  const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
+  // wgmma descriptors, built once (warp-uniform): Q and dO of the warpgroup, K / V of ring stage 0 K-major (S, dP) and K
+  // MN-major (dQ); the rest are constant steps from them (desc_add, desc_stage)
+  const uint64_t dq0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW, 0));
+  const uint64_t ddo0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_DO) + wgi * 64 * SW, 0));
+  const uint64_t dk0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_K), 0));
+  const uint64_t dv0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_V), 0));
+  const uint64_t dkn0 = desc_pin(desc_mnmajor<SW>(smem_u32(smem + Cfg::OFF_K), 0, Cfg::KV_BOX));
   const bool fast = msk.fast != 0;
   const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
 
@@ -566,36 +573,39 @@ __global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dq_
   // One wait per MMA batch: S and dP of tile i + 1 in the batch of dQ += dS_i K_i would hold S, dP, dQ and both dS fragment
   // sets at once, which does not fit in 128 registers with bf16 inputs (ptxas spills and serialises the MMAs).
   mbar_wait(&bars->qd_full, 0);
-  for (int i = 0; i < T; ++i) {
-    const int st = i % NST;
-    const uint32_t ph = (i / NST) & 1;
-    const uint32_t kst = sk + st * Cfg::KV_BYTES, vst = sv + st * Cfg::KV_BYTES;
+  // The last tile (kLast) is peeled off the loop: it is the only one that can cross the sequence end (its key range ends at
+  // hi <= len), so the loop itself does not test for it.
+  RingPos<NST> cur;  // ring stage and phase parity of tile i
+  auto tile = [&](int i, auto last_c) {
+    constexpr bool kLast = decltype(last_c)::value;
+    const int st = cur.st;
     const int n0 = (t0 + i) * BN;
     float s[BN / 2], dp[BN / 2];
-    mbar_wait(&bars->k_full[st], ph);
-    mbar_wait(&bars->v_full[st], ph);
+    mbar_wait(&bars->k_full[st], cur.ph);
+    mbar_wait(&bars->v_full[st], cur.ph);
     // the last key tile may cross the sequence end: its K rows >= len are B of dQ += dS K (dS is 0 there, K may be NaN)
-    if (n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
+    if (kLast && n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
       zero_tile_rows<BN, SW, Cfg::NBOX, kBwdThreads>(smem + Cfg::OFF_K + st * Cfg::KV_BYTES, len - n0);
       fence_proxy_async_smem();
       named_bar_sync(kBarZeroRows, kBwdThreads);
     }
     wgmma_fence();
+    const uint64_t kd = desc_stage(dk0, st, Cfg::KV_BYTES), vd = desc_stage(dv0, st, Cfg::KV_BYTES);
 #pragma unroll
     for (int ks = 0; ks < D / 16; ++ks) {
       const int kb = ks * 32, bx = kb / SW, off = kb % SW;
-      wgmma_ss<BN, BF16, 0, 0>(s, desc_kmajor<SW>(sq + bx * Cfg::Q_BOX, off), desc_kmajor<SW>(kst + bx * Cfg::KV_BOX, off), ks > 0);
+      wgmma_ss<BN, BF16, 0, 0>(s, desc_add(dq0, bx * Cfg::Q_BOX + off), desc_add(kd, bx * Cfg::KV_BOX + off), ks > 0);
     }
 #pragma unroll
     for (int ks = 0; ks < D / 16; ++ks) {
       const int kb = ks * 32, bx = kb / SW, off = kb % SW;
-      wgmma_ss<BN, BF16, 0, 0>(dp, desc_kmajor<SW>(sdo + bx * Cfg::Q_BOX, off), desc_kmajor<SW>(vst + bx * Cfg::KV_BOX, off), ks > 0);
+      wgmma_ss<BN, BF16, 0, 0>(dp, desc_add(ddo0, bx * Cfg::Q_BOX + off), desc_add(vd, bx * Cfg::KV_BOX + off), ks > 0);
     }
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(s);
     fence_regs(dp);
-    release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i);
+    release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i, st);
     __syncwarp();
 
     // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2.  The mask case is chosen once per
@@ -644,20 +654,23 @@ __global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dq_
       }
     }
     wgmma_fence();
+    const uint64_t kn = desc_stage(dkn0, st, Cfg::KV_BYTES);
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk) {
-      const uint64_t kd = desc_mnmajor<SW>(kst, kk * 16, Cfg::KV_BOX);
-      wgmma_rs<D, BF16, 1>(dq, a_hi[kk], kd, 1);
-      if constexpr (BF16) wgmma_rs<D, BF16, 1>(dq, a_lo[kk], kd, 1);
+      wgmma_rs<D, BF16, 1>(dq, a_hi[kk], desc_add(kn, kk * 16 * SW), 1);
+      if constexpr (BF16) wgmma_rs<D, BF16, 1>(dq, a_lo[kk], desc_add(kn, kk * 16 * SW), 1);
     }
     wgmma_commit();
     wgmma_wait<0>();  // an MMA batch never stays in flight across the elementwise code (ptxas would serialise them)
     fence_regs(dq);
     fence_regs(a_hi);
     fence_regs(a_lo);
-    release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i);
+    release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i, st);
     __syncwarp();
-  }
+    cur.advance();
+  };
+  for (int i = 0; i < T - 1; ++i) tile(i, std::false_type{});
+  tile(T - 1, std::true_type{});
 
   // ---------------- epilogue: dQ * alpha / (2N) -> global ----------------
 #pragma unroll

@@ -35,6 +35,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "attn_fp16_operands.cuh"
 #include "common.cuh"
@@ -160,9 +161,8 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
   }
   __syncthreads();
 
-  // TMA issue of key tile i into its K or V stage (tm = &p.tmK / &p.tmV, off = Cfg::OFF_K / OFF_V, full = its full barriers)
-  auto load = [&](const CUtensorMap* tm, int off, uint64_t* full, int i) {
-    const int st = i % NST;
+  // TMA issue of key tile i into its K or V stage st (tm = &p.tmK / &p.tmV, off = Cfg::OFF_K / OFF_V, full = its full barriers)
+  auto load = [&](const CUtensorMap* tm, int off, uint64_t* full, int i, int st) {
     mbar_arrive_expect_tx(&full[st], Cfg::KV_BYTES);
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx)
@@ -172,8 +172,9 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
   // Thread 0 loads Q and the first STAGES key tiles.  Afterwards nobody waits for a free stage: each warp releases the K (V)
   // stage of tile i once its MMAs that read it have completed, and the warp whose release is the last of the eight issues
   // the load of tile i + STAGES into it, so neither warpgroup holds the other back.
-  auto release = [&](const CUtensorMap* tm, int off, uint64_t* full, uint32_t* ctr, int i) {
-    if (lane == 0 && i + NST < T && release_is_last<kFwdThreads / 32>(&ctr[i % NST])) load(tm, off, full, i + NST);
+  // (st: the stage of tile i, i % NST)
+  auto release = [&](const CUtensorMap* tm, int off, uint64_t* full, uint32_t* ctr, int i, int st) {
+    if (lane == 0 && i + NST < T && release_is_last<kFwdThreads / 32>(&ctr[st])) load(tm, off, full, i + NST, st);
   };
   if (tid == 0) {
     prefetch_tensormap(&p.tmQ);
@@ -185,20 +186,21 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
       tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::BOX_COLS, h,
                   kDelta ? b * p.delta + m0 : (int)(row0 + m0));
     for (int i = 0; i < min(T, NST); ++i) {
-      load(&p.tmK, Cfg::OFF_K, bars->k_full, i);
-      load(&p.tmV, Cfg::OFF_V, bars->v_full, i);
+      load(&p.tmK, Cfg::OFF_K, bars->k_full, i, i);
+      load(&p.tmV, Cfg::OFF_V, bars->v_full, i, i);
     }
   }
   __syncwarp();
 
-  const int wgi = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
+  // (delta: the plain index; the descriptors held in registers through its loop would spill at d = 64 with bf16 inputs)
+  const int wgi = kDelta ? warp >> 2 : warpgroup_index(), w = warp & 3, g = lane >> 2, t4 = lane & 3;
   if constexpr (kDelta) {
     if (wgi * 64 >= mrows) {
       // a warpgroup of padding rows only: no MMA, no tanh, no output.  It still releases every stage use, once that use has
       // landed (its full barrier), so that its releases cannot run ahead into the next use of the stage and complete a
       // release while another warp still reads it; and it helps zero the V rows past the sequence end (CTA-wide barrier)
       mbar_wait(&bars->k_full[0], 0);
-      release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, 0);
+      release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, 0, 0);
       for (int i = 0; i < T; ++i) {
         const int st = i % NST;
         const bool next = i + 1 < T;
@@ -211,8 +213,8 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
         }
         if (next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
         __syncwarp();
-        release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i);
-        if (next) release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i + 1);
+        release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i, st);
+        if (next) release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i + 1, (i + 1) % NST);
         __syncwarp();
       }
       return;
@@ -221,8 +223,11 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
   const int q_base = p0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
   // delta: a warp whose 16 rows all lie past delta skips the elementwise stage (warp-uniform)
   const bool rows_idle = kDelta && wgi * 64 + w * 16 >= mrows;
-  const uint32_t sq = smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW;
-  const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
+  // wgmma descriptors, built once: Q of the warpgroup, and K (K-major) and V (MN-major) of ring stage 0; everything else is
+  // a constant step from them (desc_add), and all three are warp-uniform
+  const uint64_t dq0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW, 0));
+  const uint64_t dk0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_K), 0));
+  const uint64_t dv0 = desc_pin(desc_mnmajor<SW>(smem_u32(smem + Cfg::OFF_V), 0, Cfg::KV_BOX));
   const bool fast = msk.fast != 0;
   const int full_lim = fast ? min(p0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
   // scaled fp16 operands: S holds 2^(e_q + e_k) S, P is formed as 2^e_p P and O holds 2^(e_p + e_v) O
@@ -245,13 +250,13 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
 #pragma unroll
     for (int r = 0; r < 4; ++r) a_hi[kk][r] = a_lo[kk][r] = 0u;
   float s[BN / 2];
-  // S = Q K_i^T into s (issue only; the caller fences, commits and waits)
-  auto issue_s = [&](int i) {
-    const uint32_t kst = sk + (i % NST) * Cfg::KV_BYTES;
+  // S = Q K^T of the key tile in stage st into s (issue only; the caller fences, commits and waits)
+  auto issue_s = [&](int st) {
+    const uint64_t kd = desc_stage(dk0, st, Cfg::KV_BYTES);
 #pragma unroll
     for (int ks = 0; ks < D / 16; ++ks) {
       const int kb = ks * 32, bx = kb / SW, off = kb % SW;
-      wgmma_ss<BN, BF16, 0, 0>(s, desc_kmajor<SW>(sq + bx * Cfg::Q_BOX, off), desc_kmajor<SW>(kst + bx * Cfg::KV_BOX, off), ks > 0);
+      wgmma_ss<BN, BF16, 0, 0>(s, desc_add(dq0, bx * Cfg::Q_BOX + off), desc_add(kd, bx * Cfg::KV_BOX + off), ks > 0);
     }
   };
   mbar_wait(&bars->q_full, 0);
@@ -261,13 +266,18 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
   wgmma_commit();
   wgmma_wait<0>();
   fence_regs(s);
-  release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, 0);
+  release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, 0, 0);
   __syncwarp();
   // Per tile i (s holds S_i): P_i -> A fragments; one MMA batch of O += P_i V_i and (kMerge) S_{i+1} = Q K_{i+1}^T; one wait;
   // V_i and K_{i+1} are released.  O is never read inside the loop, so no MMA waits on the elementwise code of its own tile.
-  for (int i = 0; i < T; ++i) {
-    const int st = i % NST;
-    const bool next = i + 1 < T;
+  // The last tile (kLast) is peeled off the loop: it has no next tile, and it is the only one that can cross the sequence
+  // end (its key range ends at hi <= len), so the loop itself tests neither.
+  RingPos<NST> cur;  // ring stage and phase parity of tile i
+  auto tile = [&](int i, auto last_c) {
+    constexpr bool kLast = decltype(last_c)::value;
+    RingPos<NST> nx = cur;  // tile i + 1
+    nx.advance();
+    const int st = cur.st;
     const int n0 = (t0 + i) * BN;
     // P = silu(alpha S) * mask.  The mask case is chosen once per tile, outside the score loops, so that each loop is one
     // basic block and ptxas can overlap the tanh of independent scores instead of waiting out each one in turn.
@@ -311,40 +321,43 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
         a_lo[kk][0] = x0.lo; a_lo[kk][1] = x1.lo; a_lo[kk][2] = x2.lo; a_lo[kk][3] = x3.lo;
       }
     }
-    mbar_wait(&bars->v_full[st], (i / NST) & 1);
+    mbar_wait(&bars->v_full[st], cur.ph);
     // the last tile may cross the sequence end: its V rows >= len belong to the next sequence (P is 0 there, V may be NaN)
-    if (n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
+    if (kLast && n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
       zero_tile_rows<BN, SW, Cfg::NBOX, kFwdThreads>(smem + Cfg::OFF_V + st * Cfg::KV_BYTES, len - n0);
       fence_proxy_async_smem();
       named_bar_sync(kBarZeroRows, kFwdThreads);
     }
-    if (kMerge && next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+    if (kMerge && !kLast) mbar_wait(&bars->k_full[nx.st], nx.ph);
     wgmma_fence();
+    const uint64_t vd = desc_stage(dv0, st, Cfg::KV_BYTES);
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk) {
-      const uint64_t vd = desc_mnmajor<SW>(sv + st * Cfg::KV_BYTES, kk * 16, Cfg::KV_BOX);
-      wgmma_rs<D, BF16, 1>(o, a_hi[kk], vd, 1);
-      if constexpr (BF16) wgmma_rs<D, BF16, 1>(o, a_lo[kk], vd, 1);
+      wgmma_rs<D, BF16, 1>(o, a_hi[kk], desc_add(vd, kk * 16 * SW), 1);
+      if constexpr (BF16) wgmma_rs<D, BF16, 1>(o, a_lo[kk], desc_add(vd, kk * 16 * SW), 1);
     }
-    if (kMerge && next) issue_s(i + 1);
+    if (kMerge && !kLast) issue_s(nx.st);
     wgmma_commit();
     wgmma_wait<0>();  // an MMA batch never stays in flight across the elementwise code (ptxas would serialise them)
     fence_regs(o);
     fence_regs(a_hi);
     fence_regs(a_lo);
     fence_regs(s);
-    release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i);
-    if (!kMerge && next) {
-      mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+    release(&p.tmV, Cfg::OFF_V, bars->v_full, bars->v_free, i, st);
+    if (!kMerge && !kLast) {
+      mbar_wait(&bars->k_full[nx.st], nx.ph);
       wgmma_fence();
-      issue_s(i + 1);
+      issue_s(nx.st);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(s);
     }
-    if (next) release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i + 1);
+    if (!kLast) release(&p.tmK, Cfg::OFF_K, bars->k_full, bars->k_free, i + 1, nx.st);
     __syncwarp();
-  }
+    cur = nx;
+  };
+  for (int i = 0; i < T - 1; ++i) tile(i, std::false_type{});
+  tile(T - 1, std::true_type{});
 
   // ---------------- epilogue: O * 1/N -> global ----------------
   if constexpr (kDelta) {  // row (local row lr) of out, or with more than one chunk the unscaled fp32 partial

@@ -145,6 +145,38 @@ __device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile_addr, uint32_t k0
   return make_desc(tile_addr + k0_rows * SW, box_stride, 8 * SW, swizzle_mode(SW));
 }
 
+// The descriptor of the same operand `bytes` further on (another K slice, box or ring stage): the start-address field holds
+// addr >> 4 in the low bits, and the tiles of one CTA lie inside the 256 KB that the field spans, so the step never carries
+// out of it.  Lets a kernel build each descriptor once and step it with one 64-bit add.
+__device__ __forceinline__ uint64_t desc_add(uint64_t desc, uint32_t bytes) {
+  return (desc & 0xffffffff00000000ull) | (uint32_t)((uint32_t)desc + (bytes >> 4));  // a 32-bit add: no carry to propagate
+}
+// Hides how a descriptor was computed, so that the compiler keeps the value (in a uniform register when it is warp-uniform)
+// instead of rebuilding it from the shared-memory base inside the tile loop.
+__device__ __forceinline__ uint64_t desc_pin(uint64_t desc) {
+  asm volatile("" : "+l"(desc));
+  return desc;
+}
+// The same operand in stage st (>= 0) of a ring of stage_bytes-byte stages.
+__device__ __forceinline__ uint64_t desc_stage(uint64_t desc, int st, uint32_t stage_bytes) {
+  return (desc & 0xffffffff00000000ull) | (uint32_t)((uint32_t)desc + (uint32_t)st * (stage_bytes >> 4));
+}
+
+// Warpgroup index of the calling thread, broadcast from lane 0 so that the compiler knows it is warp-uniform and keeps what
+// is derived from it (shared-memory descriptors) in uniform registers.
+__device__ __forceinline__ int warpgroup_index() { return __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0); }
+
+// Position in a ring of NST stages, carried through a loop: stage index and mbarrier phase parity, advanced without a
+// division.
+template <int NST>
+struct RingPos {
+  int st = 0;
+  uint32_t ph = 0;
+  __device__ __forceinline__ void advance() {
+    if (++st == NST) st = 0, ph ^= 1u;
+  }
+};
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

@@ -8,7 +8,9 @@ one JSON line per wgmma attention kernel: its registers, spill stores / loads (b
 MUFU.TANH instructions in one basic block of its SASS (`cuobjdump -sass`).  A block ends at a branch and starts at a branch
 target.  The elementwise stage of these kernels issues one tanh per score; when a per-score branch splits the stage into
 one block per score, tanh_per_block is 1 and every warp waits out the full MUFU latency once per score, since nothing
-independent is left in the block to issue in between.
+independent is left in the block to issue in between.  `iter_instrs` is what one thread issues in one steady-state tile
+iteration on the full-tile path, spin loops counted once (iter_instrs below): the tanh block plus the ring, descriptor and
+branch bookkeeping around the MMAs.
 """
 import argparse
 import concurrent.futures
@@ -91,6 +93,98 @@ def max_tanh_per_block(sass):
     return best
 
 
+def _blocks(sass):
+    """Basic blocks of one function's listing: [(first address, [instruction text]), ...] in address order, and the successor
+    addresses of each block (taken branch targets and, unless the block ends in an unpredicated branch or exit, the next
+    block)."""
+    ins = []
+    for line in sass.splitlines():
+        m = re.match(r"\s*/\*([0-9a-f]{4,})\*/\s+(.*?)\s*;", line)
+        if m and not m.group(2).startswith("NOP"):
+            ins.append((int(m.group(1), 16), m.group(2)))
+    starts, ends = {ins[0][0]} if ins else set(), set()
+    for i, (addr, text) in enumerate(ins):
+        op = re.sub(r"^@!?U?P[T0-9]+\s+", "", text).split()[0].split(".")[0]
+        if op in _CTRL and op != "BSSY":
+            starts.update(int(t, 16) for t in re.findall(r"0x([0-9a-f]+)", text) if op != "CALL")
+            ends.add(addr)
+    blocks = []
+    for addr, text in ins:
+        if addr in starts or not blocks or blocks[-1][1][-1][0] in ends:
+            blocks.append((addr, []))
+        blocks[-1][1].append((addr, text))
+    succ = {}
+    for i, (first, body) in enumerate(blocks):
+        text = body[-1][1]
+        op = re.sub(r"^@!?U?P[T0-9]+\s+", "", text).split()[0].split(".")[0]
+        s = []
+        if op in ("BRA", "BRX", "JMP", "JMX"):
+            s = [int(t, 16) for t in re.findall(r"0x([0-9a-f]+)", text)]
+        falls = text.startswith("@") or op not in ("BRA", "BRX", "JMP", "JMX", "EXIT", "RET")
+        if falls and i + 1 < len(blocks):
+            s.append(blocks[i + 1][0])
+        succ[first] = s
+    return [(first, [t for _, t in body]) for first, body in blocks], succ
+
+
+def iter_instrs(sass):
+    """Instructions one thread issues in one steady-state iteration of the tile loop, on the path through the elementwise
+    block of the most MUFU.TANH (the full-tile path, where no score is masked).  The tile loop is the smallest loop that holds
+    that block.  Inside it every back edge is dropped, so that a spin loop (an mbarrier wait) counts once, and the iteration
+    is the path from the loop head through that block to the back edge with the most HGMMA (every MMA of a tile: not the
+    last tile, which issues no MMA for the next one), and of those the one of the fewest instructions: branches taken only
+    by some warps or on some tiles (the refill, the mask cases, the zeroing of rows past the sequence end) are not on it.
+    None when there is no such loop."""
+    blocks, succ = _blocks(sass)
+    tanh = {a: sum("MUFU.TANH" in t for t in body) for a, body in blocks}
+    if not tanh or max(tanh.values()) == 0:
+        return None
+    best_t = max(tanh.values())
+    targets = [a for a in tanh if tanh[a] == best_t]
+    pred = {a: [] for a, _ in blocks}
+    for a, s in succ.items():
+        for b in s:
+            if b in pred:
+                pred[b].append(a)
+    loops = []  # (nodes, head, tail) of each back edge tail -> head
+    for a, s in succ.items():
+        for head in s:
+            if head <= a and head in pred:
+                nodes, stack = {head, a}, [a]
+                while stack:
+                    for p in pred[stack.pop()]:
+                        if p not in nodes:
+                            nodes.add(p)
+                            stack.append(p)
+                if any(t in nodes for t in targets):
+                    loops.append((nodes, head, a))
+    if not loops:
+        return None
+    nodes, head, tail = min(loops, key=lambda x: len(x[0]))
+
+    # a path's cost is (-HGMMA, instructions), least first; both ends counted
+    cost = {a: (-sum(t.startswith("HGMMA") for t in body), len(body)) for a, body in blocks}
+
+    def add(x, y, sign=1):
+        return (x[0] + sign * y[0], x[1] + sign * y[1])
+
+    def dist_from(src, forward):  # least cost of a forward (address-increasing) path inside the loop from / to src
+        d = {src: cost[src]}
+        for a in sorted(nodes, reverse=not forward):
+            if a not in d:
+                continue
+            nxt = [b for b in succ[a] if b in nodes and b > a] if forward else [p for p in pred[a] if p in nodes and p < a]
+            for b in nxt:
+                c = add(d[a], cost[b])
+                if b not in d or c < d[b]:
+                    d[b] = c
+        return d
+
+    down, up = dist_from(head, True), dist_from(tail, False)
+    paths = [add(add(down[t], up[t]), cost[t], -1) for t in targets if t in down and t in up]
+    return min(paths)[1] if paths else None
+
+
 def _sass_by_function(text):
     funcs, name, buf = {}, None, []
     for line in text.splitlines():
@@ -138,7 +232,8 @@ def report(kernel_filter="wgmma_kernel"):
             name = subprocess.run([cufilt, mangled], capture_output=True, text=True, check=True).stdout.strip()
             if kernel_filter not in name:
                 continue
-            res[name] = {**info.get(mangled, {"notes": []}), "tanh_per_block": max_tanh_per_block(sass)}
+            res[name] = {**info.get(mangled, {"notes": []}), "tanh_per_block": max_tanh_per_block(sass),
+                         "iter_instrs": iter_instrs(sass)}
     return res
 
 
