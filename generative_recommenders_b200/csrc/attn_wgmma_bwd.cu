@@ -1,5 +1,5 @@
 // Jagged HSTU attention backward on the Hopper warpgroup tensor cores (wgmma) with TMA-staged tiles.  bf16 / fp16,
-// dqk == dv in {32, 64, 128}.
+// dqk == dv in {32, 64, 128, 256}.
 //
 // One CTA per (128-row KEY tile, head, sequence); early key tiles (the heavy ones under a causal mask) are scheduled first.
 // K and V of the tile stay in shared memory; the CTA streams the 64-row query tiles that can attend to it (Q_j and dO_j,
@@ -34,8 +34,13 @@
 // Every dq / dk / dv element is then summed by one thread in a fixed order, so the result is bitwise reproducible.
 // At d = 32 recomputing S and dP costs two MMA units per score against the eight that the whole backward issues, while the
 // elementwise work per score is the same; at larger d the recomputed MMAs weigh more and the fused kernel stays the default.
-// The split kernels run two CTAs per SM at d = 32 and one at d = 64 / 128 (their accumulators need more than 128
-// registers per thread there); bf16 at d = 64 / 128 keeps the hi + lo operand pairs.
+// The split kernels run two CTAs per SM at d = 32 and one at d = 64 / 128 / 256 (their accumulators need more than 128
+// registers per thread there); bf16 at d >= 64 keeps the hi + lo operand pairs.
+// d = 256 always runs the split kernels (a fused dQ accumulator would be L * H * 1 KB of fp32), except that a deterministic
+// backward there stays on the generic kernels.  Full-width dK + dV would take 256 registers per thread, so two CTAs share
+// each key tile, one 128-column half of dK / dV each (bwd_key_tile's DN), and both compute S^T / dP^T over all 256 columns;
+// with K and V taking 128 KB, the query tiles are 32 rows in a 3-stage ring.  The dQ kernel keeps the full width on 32-key
+// tiles (3 stages).
 //
 // Reference math: ops/triton/triton_hstu_attention.py:995-1006,1222 and SURVEY.md appendix A; unlike the Triton
 // kernel dQ is accumulated in fp32, not in the input dtype (triton_attention_utils.py:47-60).
@@ -90,15 +95,20 @@ struct BwdScales {
   }
 };
 
-// CTAs per SM of the split kernels: two at d = 32 (<= 128 registers per thread), one at d = 64 / 128
+// CTAs per SM of the split kernels: two at d = 32 (<= 128 registers per thread), one at d = 64 / 128 / 256
 constexpr int split_min_blocks(int d) { return d == 32 ? 2 : 1; }
 constexpr int kSmemPerSm = 232448;  // dynamic shared memory one CTA may use on sm_90
+// dK / dV columns one CTA of the dK / dV kernel accumulates: all of them, except at d = 256, where 64 + 64 fp32 accumulators
+// of full width would take 256 registers per thread; there two CTAs per key tile take one 128-column half each
+__host__ __device__ constexpr int dkdv_cols(int d) { return d == 256 ? 128 : d; }
 
 // FUSED_DQ: the key-tile kernel also computes dQ (dS buffers in shared memory); without it the layout ends after the ring,
-// which then has four stages at every d (d = 128: 192 KB, one CTA per SM)
+// which then has four stages (d = 128: 192 KB, one CTA per SM), or at d = 256, where K and V alone take 128 KB, three
+// stages of 32 query rows (224 KB)
 template <int D, bool FUSED_DQ = true>
 struct BwdCfg {
-  static constexpr int BKV = 128, BQ = 64;
+  static constexpr int BKV = 128;
+  static constexpr int BQ = D == 256 ? 32 : 64;  // query rows per streamed tile
   static constexpr int SW = (D * 2 >= 128) ? 128 : D * 2;
   static constexpr int BOX_COLS = SW / 2;
   static constexpr int NBOX = D / BOX_COLS;
@@ -106,7 +116,7 @@ struct BwdCfg {
   static constexpr int QD_BOX = BQ * SW;
   static constexpr int KV_BYTES = BKV * D * 2;
   static constexpr int QD_BYTES = BQ * D * 2;
-  static constexpr int STAGES = (D <= 32 || !FUSED_DQ) ? 4 : (D == 64 ? 3 : 2);  // Q_j / dO_j ring depth
+  static constexpr int STAGES = D == 256 ? 3 : (D <= 32 || !FUSED_DQ) ? 4 : (D == 64 ? 3 : 2);  // Q_j / dO_j ring depth
   static constexpr int DS_BYTES = BKV * BQ * 2;                      // one [128 kv][64 q] box, 128-byte swizzle
   static constexpr int DQN = D < 64 ? D : 64;                        // dQ columns per pass (one 128-byte box of K)
   static constexpr int OFF_K = 0;
@@ -134,13 +144,17 @@ struct QTiles {
 
 // Body of the key-stationary kernels: FUSED_DQ = attn_bwd_wgmma_kernel (dK, dV and the dQ atomics), otherwise
 // attn_bwd_dkdv_wgmma_kernel (dK and dV only; the warpgroups meet at the ring and once at the query tile that crosses the
-// sequence end).
-template <int D, bool BF16, bool FUSED_DQ>
+// sequence end).  DN: the dK / dV columns the CTA accumulates.  With DN < D, D / DN CTAs share a key tile: CTA x takes key
+// tile x / (D / DN) and columns [c0, c0 + DN), c0 = DN (x % (D / DN)); its S^T / dP^T MMAs still reduce over all D columns.
+template <int D, bool BF16, bool FUSED_DQ, int DN = D>
 __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   using Cfg = BwdCfg<D, FUSED_DQ>;
   constexpr int SW = Cfg::SW, BQ = Cfg::BQ, NST = Cfg::STAGES;
+  constexpr int NSL = D / DN;  // column slices per key tile
+  static_assert(DN % Cfg::BOX_COLS == 0 && (DN == D || !FUSED_DQ), "a slice is whole boxes, and only of the dK / dV kernel");
   const int b = blockIdx.z, h = blockIdx.y;
-  const int n0 = blockIdx.x * Cfg::BKV;
+  const int n0 = (blockIdx.x / NSL) * Cfg::BKV;
+  const int c0 = (blockIdx.x % NSL) * DN;
   const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
   int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
   if (len > p.max_seq_len) {  // rows past max_seq_len get zero gradients
@@ -210,18 +224,21 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
   const uint32_t sq = smem_u32(smem + Cfg::OFF_Q), sdo = smem_u32(smem + Cfg::OFF_DO);
   const uint32_t sds = smem_u32(smem + Cfg::OFF_DS);
+  // Q_j / dO_j columns [c0, c0 + DN) as B of dK / dV: whole boxes from box c0 / BOX_COLS on
+  const uint32_t sq_c = sq + c0 / Cfg::BOX_COLS * Cfg::QD_BOX, sdo_c = sdo + c0 / Cfg::BOX_COLS * Cfg::QD_BOX;
   const bool fast = msk.fast != 0;
   // keys of this tile that every query row >= q_full_from may attend (fast mask): all of them are history keys below the row
   const bool keys_hist = !msk.has_tgt || n0 + Cfg::BKV <= msk.max_id;
 
   constexpr bool kScaled = !BF16 && !FUSED_DQ && D == 32;  // the d = 32 dK / dV kernel also runs bf16 inputs on fp16 copies
   const BwdScales sc(p, b, h, D);
-  float dv[D / 2], dk[D / 2];
+  constexpr int KQ = BQ / 16;  // k16 slices of a query tile (A fragments of P^T / dS^T)
+  float dv[DN / 2], dk[DN / 2];
 #pragma unroll
-  for (int e = 0; e < D / 2; ++e) dv[e] = dk[e] = 0.f;
-  uint32_t pf_hi[4][4], pf_lo[4][4], df_hi[4][4], df_lo[4][4];
+  for (int e = 0; e < DN / 2; ++e) dv[e] = dk[e] = 0.f;
+  uint32_t pf_hi[KQ][4], pf_lo[KQ][4], df_hi[KQ][4], df_lo[KQ][4];
 #pragma unroll
-  for (int kk = 0; kk < 4; ++kk)
+  for (int kk = 0; kk < KQ; ++kk)
 #pragma unroll
     for (int r = 0; r < 4; ++r) pf_hi[kk][r] = pf_lo[kk][r] = df_hi[kk][r] = df_lo[kk][r] = 0u;
 
@@ -246,7 +263,7 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
       fence_proxy_async_smem();
       named_bar_sync(kBarZeroRows, kBwdThreads);
     }
-    float s[32], dp[32];
+    float s[BQ / 2], dp[BQ / 2];
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < D / 16; ++ks) {
@@ -330,7 +347,7 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
       // dV += P^T dO_j issued as soon as P is packed, then dK += dS^T Q_j: P^T and dS^T are never both held in fp32 next to
       // both fragment sets, which keeps a bf16 thread at 128 registers without wgmma serialisation (ptxas C7512)
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
+      for (int kk = 0; kk < KQ; ++kk)
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
           const Operand<BF16> pp(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
@@ -338,14 +355,14 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
         }
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint64_t dod = desc_mnmajor<SW>(sdo + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
-        wgmma_rs<D, BF16, 1>(dv, pf_hi[kk], dod, 1);
-        if constexpr (BF16) wgmma_rs<D, BF16, 1>(dv, pf_lo[kk], dod, 1);
+      for (int kk = 0; kk < KQ; ++kk) {
+        const uint64_t dod = desc_mnmajor<SW>(sdo_c + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
+        wgmma_rs<DN, BF16, 1>(dv, pf_hi[kk], dod, 1);
+        if constexpr (BF16) wgmma_rs<DN, BF16, 1>(dv, pf_lo[kk], dod, 1);
       }
       wgmma_commit();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
+      for (int kk = 0; kk < KQ; ++kk)
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
           const Operand<BF16> dd(dp[8 * kk + 2 * r], dp[8 * kk + 2 * r + 1]);
@@ -353,10 +370,10 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
         }
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint64_t qd = desc_mnmajor<SW>(sq + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
-        wgmma_rs<D, BF16, 1>(dk, df_hi[kk], qd, 1);
-        if constexpr (BF16) wgmma_rs<D, BF16, 1>(dk, df_lo[kk], qd, 1);
+      for (int kk = 0; kk < KQ; ++kk) {
+        const uint64_t qd = desc_mnmajor<SW>(sq_c + st * Cfg::QD_BYTES, kk * 16, Cfg::QD_BOX);
+        wgmma_rs<DN, BF16, 1>(dk, df_hi[kk], qd, 1);
+        if constexpr (BF16) wgmma_rs<DN, BF16, 1>(dk, df_lo[kk], qd, 1);
       }
     }
     wgmma_commit();
@@ -419,10 +436,10 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   for (int hh = 0; hh < 2; ++hh) {
     const int kj = k_base + hh * 8;
     if (kj < len) {
-      uint16_t* krow = reinterpret_cast<uint16_t*>(p.dk) + (row0 + kj) * p.dk_row_stride + (long long)h * p.dk_head_stride + 2 * t4;
-      uint16_t* vrow = reinterpret_cast<uint16_t*>(p.dv) + (row0 + kj) * p.dv_row_stride + (long long)h * p.dv_head_stride + 2 * t4;
+      uint16_t* krow = reinterpret_cast<uint16_t*>(p.dk) + (row0 + kj) * p.dk_row_stride + (long long)h * p.dk_head_stride + c0 + 2 * t4;
+      uint16_t* vrow = reinterpret_cast<uint16_t*>(p.dv) + (row0 + kj) * p.dv_row_stride + (long long)h * p.dv_head_stride + c0 + 2 * t4;
 #pragma unroll
-      for (int nb = 0; nb < D / 8; ++nb) {
+      for (int nb = 0; nb < DN / 8; ++nb) {
         float k0 = dk[nb * 4 + hh * 2] * p.dk_scale, k1 = dk[nb * 4 + hh * 2 + 1] * p.dk_scale;
         float v0 = dv[nb * 4 + hh * 2] * p.dv_scale, v1 = dv[nb * 4 + hh * 2 + 1] * p.dv_scale;
         if (kScaled) {
@@ -442,17 +459,18 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __
   bwd_key_tile<D, BF16, true>(p);
 }
 
-// d = 32: two CTAs per SM (<= 128 registers per thread, 49 KB of shared memory)
+// d = 32: two CTAs per SM (<= 128 registers per thread, 49 KB of shared memory); d = 256: one 128-column half per CTA
 template <int D, bool BF16>
 __global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dkdv_wgmma_kernel(const __grid_constant__ BwdParams p) {
-  bwd_key_tile<D, BF16, false>(p);
+  bwd_key_tile<D, BF16, false, dkdv_cols(D)>(p);
 }
 
 // ---------------- dQ, query-stationary (split path) ----------------
 template <int D>
 struct DqCfg {
   static constexpr int BM = 128;  // query rows per CTA (two warpgroups of 64)
-  static constexpr int BN = 64;   // key rows per tile
+  // key rows per tile; d = 256: Q and dO take 128 KB, so three stages of 32 keys (224 KB) and the full-width dQ accumulator
+  static constexpr int BN = D == 256 ? 32 : 64;
   static constexpr int SW = (D * 2 >= 128) ? 128 : D * 2;
   static constexpr int BOX_COLS = SW / 2;
   static constexpr int NBOX = D / BOX_COLS;
@@ -460,7 +478,7 @@ struct DqCfg {
   static constexpr int KV_BOX = BN * SW;
   static constexpr int Q_BYTES = BM * D * 2;
   static constexpr int KV_BYTES = BN * D * 2;
-  static constexpr int STAGES = 3;  // K / V ring depth (d = 128: 161 KB, one CTA per SM)
+  static constexpr int STAGES = 3;  // K / V ring depth (d = 128: 161 KB, d = 256: 225 KB, one CTA per SM)
   static constexpr int OFF_Q = 0;
   static constexpr int OFF_DO = OFF_Q + Q_BYTES;
   static constexpr int OFF_K = OFF_DO + Q_BYTES;
@@ -717,8 +735,8 @@ __global__ void dq_convert_kernel(const float* __restrict__ acc, uint16_t* __res
 // ------------------------------------------------------------------------------------------------
 static bool wgmma_bwd_supported(const hstu_attn_params& p) {
   if (!wgmma_fwd_supported(p)) return false;  // dtype / dims / alignment of q, k, v (out is not used by the backward)
-  // d = 256: dK and dV alone would take all the registers of a consumer thread; the backward runs on the generic path
-  if (p.dqk != 32 && p.dqk != 64 && p.dqk != 128) return false;
+  // d = 256 runs the split kernels (dK / dV in column halves); a deterministic backward there stays on the generic kernels
+  if (p.dqk == 256 && p.deterministic) return false;
   return aligned_view(p.dout, p.do_row_stride, p.do_head_stride) && aligned_view(p.dq, p.dq_row_stride, p.dq_head_stride) &&
          aligned_view(p.dk, p.dk_row_stride, p.dk_head_stride) && aligned_view(p.dv_out, p.dv_row_stride, p.dv_head_stride);
 }
@@ -732,9 +750,9 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd) {
   return wgmma_bwd_supported(q);
 }
 
-// d = 32, or a deterministic backward: dK / dV and dQ in two kernels, without atomics or dQ workspace; otherwise the fused
-// kernel (DESIGN.md 3.2)
-static bool split_dq(const hstu_attn_params& p) { return p.dqk == 32 || p.deterministic != 0; }
+// d = 32 / 256, or a deterministic backward: dK / dV and dQ in two kernels, without atomics or dQ workspace; otherwise the
+// fused kernel (DESIGN.md 3.2).  At d = 256 the fused kernel's fp32 dQ accumulator would be L * H * 1 KB.
+static bool split_dq(const hstu_attn_params& p) { return p.dqk == 32 || p.dqk == 256 || p.deterministic != 0; }
 
 // bf16 at d = 32: the fp16 kernels on exactly scaled copies (attn_fp16_operands.cu)
 static bool fp16_copies(const hstu_attn_params& p) { return p.dtype == HSTU_BF16 && p.dqk == 32; }
@@ -794,9 +812,11 @@ static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp
   if constexpr (kSplit) {
     auto kdkdv = attn_bwd_dkdv_wgmma_kernel<D, BF16>;
     HSTU_CUDA_OK(cudaFuncSetAttribute(kdkdv, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    kdkdv<<<dim3((p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV, p.heads, p.batch), kBwdThreads, Cfg::SMEM_BYTES, st>>>(bp);
+    // the column slices of one key tile are adjacent CTAs (they read the same K, V and query tiles)
+    const int key_ctas = (p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV * (D / dkdv_cols(D));
+    kdkdv<<<dim3(key_ctas, p.heads, p.batch), kBwdThreads, Cfg::SMEM_BYTES, st>>>(bp);
     HSTU_CUDA_OK(cudaGetLastError());
-    // the dQ kernel tiles 128 query rows and 64 key rows
+    // the dQ kernel tiles 128 query rows and 64 key rows (32 at d = 256)
     using QC = DqCfg<D>;
     if (int e = make_tmap_rows_heads(&bp.tmQ, src[0], p.total_rows, p.heads, D, rs[0], hs[0], QC::BOX_COLS, QC::BM)) return e;
     if (int e = make_tmap_rows_heads(&bp.tmK, src[1], p.total_rows, p.heads, D, rs[1], hs[1], QC::BOX_COLS, QC::BN)) return e;
@@ -839,6 +859,8 @@ int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st) {
     case 128:
       if (split) return bf ? launch_bwd_wgmma<128, true, true>(p, st) : launch_bwd_wgmma<128, false, true>(p, st);
       return bf ? launch_bwd_wgmma<128, true, false>(p, st) : launch_bwd_wgmma<128, false, false>(p, st);
+    case 256:  // split only (split_dq)
+      return bf ? launch_bwd_wgmma<256, true, true>(p, st) : launch_bwd_wgmma<256, false, true>(p, st);
   }
   set_error("wgmma backward: unsupported head dim %d", p.dqk);
   return HSTU_ERR_UNSUPPORTED;

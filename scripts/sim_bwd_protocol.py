@@ -176,7 +176,8 @@ def run(T, d, seed, break_ds=False, straddle=True, break_zero=False):
     return _simulate({f"W{w}": W(w) for w in range(WARPS)}, B, rnd)
 
 
-DKDV_STAGES = 4  # BwdCfg<D, false>::STAGES (every d)
+DKDV_STAGES = 4  # BwdCfg<D, false>::STAGES at d <= 128
+DKDV_STAGES_D256 = 3  # BwdCfg<256, false>::STAGES (32-row query tiles next to 128 KB of K and V)
 
 
 def run_dkdv(T, seed, break_release=False, first_releaser=False, early_release=False, straddle=True, break_zero=False,
