@@ -1,0 +1,482 @@
+// Jagged HSTU attention forward on the Hopper warpgroup tensor cores (wgmma) with TMA-staged tiles: the kernel body and its
+// launcher, shared by attn_wgmma_fwd.cu (dqk == dv in {32, 64, 128, 256}) and attn_wgmma_mixed_fwd.cu (dqk < dv, both in
+// that set).  bf16 / fp16.  Two widths: DQK, of Q and K and the reduction of S = Q K^T, and DV, of V and O (the N of P V).
+// Q / K and V are TMA boxes of their own swizzle width; every existing instantiation is DQK == DV == d.
+//
+// One CTA per (128-row query tile, head, sequence); heavy (late) query tiles are scheduled first.  Two warpgroups
+// of 64 query rows each.  Per key tile:
+//   S = Q K^T            (wgmma, A = Q and B = K both K-major in shared memory, fp32 accumulators)
+//   P = silu(alpha S) * mask   (one tanh per score, in registers)
+//   O += P V             (wgmma, A = P from registers, B = V MN-major in shared memory)
+// Key tiles of 64 rows keep a thread at <= 128 registers for d <= 64, so two CTAs share an SM there.
+// Each warpgroup waits for its own MMAs; the two warpgroups overlap each other's tensor-core and elementwise phases.  With
+// d <= 64, O += P_i V_i and S_{i+1} = Q K_{i+1}^T are one MMA batch with one wait per tile (O is never read in the loop).
+// Thread 0 issues the first TMA loads: Q, then the K and V tiles through a ring of STAGES buffers each.  Each warp releases a
+// stage once its MMAs that read it have completed, and the warp whose release is the last of the eight issues the refill
+// (release_is_last, wgmma.cuh), so no thread ever waits for a free stage and neither warpgroup holds the other back.  No
+// separate producer warp: the 64 x d fp32 O accumulator (d = 256: 128 registers per thread) needs the register budget of a
+// 256-thread block.
+// P is a 16-bit MMA operand of the same format as V (wgmma takes one format for A and B): fp16 for fp16 inputs, and for
+// bf16 inputs a hi + lo pair of bf16 operands multiplied twice (wgmma.cuh, Operand), so that its rounding stays well inside
+// the 1e-3 parity budget.  bf16 inputs at d = 32 instead run the fp16 kernel on exactly scaled fp16 copies of q, k, v with
+// a scaled fp16 P (`amax`, attn_fp16_operands.cuh); its epilogue undoes the scales and writes bf16.  The 1/N factor of the reference is applied once in the epilogue (registers -> global, rows past
+// the sequence end are not written).  Rows past the sequence end that a TMA box drags in are masked out of P, and zeroed in the
+// V stage of the one key tile that crosses the end (zero_tile_rows), since P = 0 does not neutralise a NaN or Inf in V.
+//
+// Delta-q (kDelta, KV-cached inference, DESIGN.md 3.6): query row i of sequence b is row b * delta + i of q / out, at sequence
+// position len - delta + i; keys are the whole (unclipped) sequence; no zero-fill past max_seq_len.  The grid is (sequence x
+// head, query tile, key chunk): HSTU has no softmax, so outputs over disjoint key ranges simply add.  Each CTA takes chunk c
+// of the key tiles its rows attend (an even split in whole 64-key tiles).  With one chunk it writes out itself; with more it
+// writes unscaled fp32 partials to the workspace and delta_reduce_kernel sums them in chunk order (bitwise reproducible).
+// Padding rows past delta cost nothing: a warpgroup with no valid row issues no MMA and only releases its stages once
+// they have landed (so its releases never run ahead into the next use of a stage), and a warp with no valid row skips the
+// elementwise stage with P = 0.  bf16 keeps the hi / lo split of P at every d, d = 32 included (no pre-pass over the cache).
+//
+// Reference semantics: ops/pytorch/pt_hstu_attention.py:130-171 (delta: :175-235); tile skipping mirrors the idea of
+// ops/triton/triton_hstu_attention.py:517-543 (loop bounds from the mask) but is derived from common.cuh's ranges.
+#pragma once
+#include <string.h>
+
+#include <algorithm>
+#include <type_traits>
+
+#include "attn_fp16_operands.cuh"
+#include "common.cuh"
+#include "internal.h"
+#include "wgmma.cuh"
+
+namespace hstu {
+using namespace wg;
+
+struct alignas(64) FwdParams {
+  CUtensorMap tmQ, tmK, tmV;
+  const void* seq_offsets;
+  const void* num_targets;
+  void* out;
+  long long o_row_stride, o_head_stride;
+  int offsets_i64, targets_i64;
+  int max_seq_len;
+  int win, min_full, ctx;
+  float alpha_half;  // alpha / 2
+  float inv_n;       // 1 / max_seq_len
+  const uint32_t* amax;  // fp16 kernel on scaled copies of bf16 inputs: [B, H, 4] amax bits (attn_fp16_operands.cuh); else null
+  int heads;
+  // delta-q only (kDelta): query rows per sequence, and with gridDim.z > 1 key chunks the fp32 partials [chunks, B * delta, H, DV]
+  int delta;
+  float* part;
+};
+
+template <int DQK, int DV = DQK>
+struct FwdCfg {
+  static constexpr int BM = 128;                     // query rows per CTA (two warpgroups of 64)
+  static constexpr int BN = 64;                      // key rows per tile
+  static constexpr int SW = (DQK * 2 >= 128) ? 128 : DQK * 2;  // swizzle width (bytes) of the Q / K boxes
+  static constexpr int SWV = (DV * 2 >= 128) ? 128 : DV * 2;   // and of the V boxes
+  static constexpr int BOX_COLS = SW / 2;
+  static constexpr int BOX_COLS_V = SWV / 2;
+  static constexpr int Q_BOX = BM * SW;
+  static constexpr int K_BOX = BN * SW;
+  static constexpr int V_BOX = BN * SWV;
+  static constexpr int Q_BYTES = BM * DQK * 2;
+  static constexpr int K_BYTES = BN * DQK * 2;
+  static constexpr int V_BYTES = BN * DV * 2;
+  static constexpr int NBOX = DQK / BOX_COLS;
+  static constexpr int NBOX_V = DV / BOX_COLS_V;
+  // d = 256: 64 KB of Q and 64 KB per stage; every dqk < dv pair has room for three (128, 256: 32 + 3 x 48 KB)
+  static constexpr int STAGES = (DQK == 256) ? 2 : 3;
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_K = OFF_Q + Q_BYTES;
+  static constexpr int OFF_V = OFF_K + STAGES * K_BYTES;
+  static constexpr int OFF_BAR = OFF_V + STAGES * V_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;  // + barriers + alignment slack
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+  static_assert(DQK <= DV, "dqk > dv has no instantiation");
+};
+constexpr int kFwdThreads = 256;
+// dv <= 64: two CTAs per SM (<= 128 registers per thread; the O accumulator is dv / 2 of them)
+template <int DV> constexpr int kFwdMinBlocks = (DV <= 64) ? 2 : 1;
+
+struct FwdBars {
+  uint64_t q_full;
+  uint64_t k_full[3], v_full[3];
+  uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
+};
+
+// Delta-q: the output row (of q / out, and of the partials of chunk blockIdx.z) of local query row 0 of the CTA, and the CTA's
+// valid query rows.  Recomputed from the grid where needed, so that nothing extra stays live through the key loop.
+struct DeltaRows {
+  long long out_row, part_row;
+  int rows;
+};
+template <int BM>
+__device__ __forceinline__ DeltaRows delta_rows(const FwdParams& p) {
+  const int m0 = (int)blockIdx.y * BM;
+  const long long r = (long long)(blockIdx.x / p.heads) * p.delta + m0;
+  return {r, (long long)blockIdx.z * (gridDim.x / p.heads) * p.delta + r, min(BM, p.delta - m0)};
+}
+
+// kDelta: the delta-q geometry and key chunks described at the top (grid (B * H, query tiles, chunks)); otherwise the full
+// attention of grid (query tiles, H, B).  Its only instantiations are the kernels of attn_wgmma_fwd.cu and
+// attn_wgmma_mixed_fwd.cu.
+template <int DQK, int DV, bool BF16, bool kDelta>
+__device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
+  using Cfg = FwdCfg<DQK, DV>;
+  constexpr int SW = Cfg::SW, SWV = Cfg::SWV, BN = Cfg::BN, NST = Cfg::STAGES;
+  // dv <= 64: P V of tile i and S of tile i + 1 form one MMA batch with one wait (both fit in 128 registers); larger dv waits
+  // for each batch separately, since the O accumulator leaves no room for S next to the P fragments
+  constexpr bool kMerge = DV <= 64;
+  const int b = kDelta ? (int)blockIdx.x / p.heads : (int)blockIdx.z, h = kDelta ? (int)blockIdx.x % p.heads : (int)blockIdx.y;
+  const int m0 = kDelta ? (int)blockIdx.y * Cfg::BM : (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;  // first query row of the CTA
+  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
+  int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
+  if (!kDelta && len > p.max_seq_len) {  // rows past max_seq_len are ignored on the way in and zero on the way out
+    if (blockIdx.x == 0) zero_rows(p.out, 2, p.o_row_stride, (long long)h * p.o_head_stride, DV, row0 + p.max_seq_len, row0 + len);
+    len = p.max_seq_len;
+  }
+  if (!kDelta && m0 >= len) return;
+  const int p0 = kDelta ? len - p.delta + m0 : m0;  // sequence position of query row m0 (delta: the last delta rows)
+  const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
+  const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
+  const int mrows = min(Cfg::BM, (kDelta ? p.delta : len) - m0);
+  int lo, hi;
+  kv_range_for_q_rows(msk, p0, p0 + mrows, &lo, &hi);
+  int t0 = lo / BN;
+  int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
+  if constexpr (kDelta) {
+    // chunk blockIdx.z of gridDim.z even shares of whole tiles; an empty share (or no key at all) writes zeros, so that
+    // every partial the reduction reads is defined
+    const int per = (T + (int)gridDim.z - 1) / (int)gridDim.z;
+    t0 += (int)blockIdx.z * per;
+    T = min(per, T - (int)blockIdx.z * per);
+    if (T <= 0) {
+      const DeltaRows dr = delta_rows<Cfg::BM>(p);
+      for (int idx = threadIdx.x; idx < dr.rows * DV; idx += kFwdThreads) {
+        if (gridDim.z > 1) p.part[((dr.part_row + idx / DV) * p.heads + h) * DV + idx % DV] = 0.f;
+        else reinterpret_cast<uint16_t*>(p.out)[(dr.out_row + idx / DV) * p.o_row_stride + (long long)h * p.o_head_stride + idx % DV] = 0;
+      }
+      return;
+    }
+  }
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  FwdBars* bars = reinterpret_cast<FwdBars*>(smem + Cfg::OFF_BAR);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    mbar_init(&bars->q_full, 1);
+    for (int i = 0; i < NST; ++i) {
+      mbar_init(&bars->k_full[i], 1);
+      mbar_init(&bars->v_full[i], 1);
+      bars->k_free[i] = bars->v_free[i] = 0u;
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  // TMA issue of key tile i into its K (kKey) or V (kVal) stage st
+  constexpr std::false_type kKey{};
+  constexpr std::true_type kVal{};
+  auto load = [&](auto val_c, int i, int st) {
+    constexpr bool kIsV = decltype(val_c)::value;
+    constexpr int bytes = kIsV ? Cfg::V_BYTES : Cfg::K_BYTES, box = kIsV ? Cfg::V_BOX : Cfg::K_BOX;
+    constexpr int nbox = kIsV ? Cfg::NBOX_V : Cfg::NBOX, cols = kIsV ? Cfg::BOX_COLS_V : Cfg::BOX_COLS;
+    uint64_t* full = kIsV ? bars->v_full : bars->k_full;
+    mbar_arrive_expect_tx(&full[st], bytes);
+#pragma unroll
+    for (int bx = 0; bx < nbox; ++bx)
+      tma_load_3d(smem + (kIsV ? Cfg::OFF_V : Cfg::OFF_K) + st * bytes + bx * box, kIsV ? &p.tmV : &p.tmK, &full[st], bx * cols, h,
+                  (int)(row0 + (long long)(t0 + i) * BN));
+  };
+  // Thread 0 loads Q and the first STAGES key tiles.  Afterwards nobody waits for a free stage: each warp releases the K (V)
+  // stage of tile i once its MMAs that read it have completed, and the warp whose release is the last of the eight issues
+  // the load of tile i + STAGES into it, so neither warpgroup holds the other back.
+  // (st: the stage of tile i, i % NST)
+  auto release = [&](auto val_c, int i, int st) {
+    uint32_t* ctr = decltype(val_c)::value ? bars->v_free : bars->k_free;
+    if (lane == 0 && i + NST < T && release_is_last<kFwdThreads / 32>(&ctr[st])) load(val_c, i + NST, st);
+  };
+  if (tid == 0) {
+    prefetch_tensormap(&p.tmQ);
+    prefetch_tensormap(&p.tmK);
+    prefetch_tensormap(&p.tmV);
+    mbar_arrive_expect_tx(&bars->q_full, Cfg::Q_BYTES);
+#pragma unroll
+    for (int bx = 0; bx < Cfg::NBOX; ++bx)
+      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::BOX_COLS, h,
+                  kDelta ? b * p.delta + m0 : (int)(row0 + m0));
+    for (int i = 0; i < min(T, NST); ++i) {
+      load(kKey, i, i);
+      load(kVal, i, i);
+    }
+  }
+  __syncwarp();
+
+  // (delta: the plain index; the descriptors held in registers through its loop would spill at d = 64 with bf16 inputs)
+  const int wgi = kDelta ? warp >> 2 : warpgroup_index(), w = warp & 3, g = lane >> 2, t4 = lane & 3;
+  if constexpr (kDelta) {
+    if (wgi * 64 >= mrows) {
+      // a warpgroup of padding rows only: no MMA, no tanh, no output.  It still releases every stage use, once that use has
+      // landed (its full barrier), so that its releases cannot run ahead into the next use of the stage and complete a
+      // release while another warp still reads it; and it helps zero the V rows past the sequence end (CTA-wide barrier)
+      mbar_wait(&bars->k_full[0], 0);
+      release(kKey, 0, 0);
+      for (int i = 0; i < T; ++i) {
+        const int st = i % NST;
+        const bool next = i + 1 < T;
+        const int n0 = (t0 + i) * BN;
+        mbar_wait(&bars->v_full[st], (i / NST) & 1);
+        if (n0 + BN > len) {
+          zero_tile_rows<BN, SWV, Cfg::NBOX_V, kFwdThreads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, len - n0);
+          fence_proxy_async_smem();
+          named_bar_sync(kBarZeroRows, kFwdThreads);
+        }
+        if (next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+        __syncwarp();
+        release(kVal, i, st);
+        if (next) release(kKey, i + 1, (i + 1) % NST);
+        __syncwarp();
+      }
+      return;
+    }
+  }
+  const int q_base = p0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
+  // delta: a warp whose 16 rows all lie past delta skips the elementwise stage (warp-uniform)
+  const bool rows_idle = kDelta && wgi * 64 + w * 16 >= mrows;
+  // wgmma descriptors, built once: Q of the warpgroup, and K (K-major) and V (MN-major) of ring stage 0; everything else is
+  // a constant step from them (desc_add), and all three are warp-uniform
+  const uint64_t dq0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW, 0));
+  const uint64_t dk0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_K), 0));
+  const uint64_t dv0 = desc_pin(desc_mnmajor<SWV>(smem_u32(smem + Cfg::OFF_V), 0, Cfg::V_BOX));
+  const bool fast = msk.fast != 0;
+  const int full_lim = fast ? min(p0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
+  // scaled fp16 operands: S holds 2^(e_q + e_k) S, P is formed as 2^e_p P and O holds 2^(e_p + e_v) O
+  constexpr bool kScaled = !kDelta && !BF16 && DQK == 32 && DV == 32;  // the only instantiation that runs bf16 inputs on fp16 copies
+  float c_s = p.alpha_half, c_p = 1.f;
+  int e_out = 0;
+  if (kScaled && p.amax != nullptr) {
+    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, 2.f * p.alpha_half, DQK);
+    c_s = ldexpf(p.alpha_half, -(ex.q + ex.k));
+    c_p = pow2f(ex.p);
+    e_out = -(ex.p + ex.v);
+  }
+
+  float o[DV / 2];
+#pragma unroll
+  for (int e = 0; e < DV / 2; ++e) o[e] = 0.f;
+  uint32_t a_hi[BN / 16][4], a_lo[BN / 16][4];
+#pragma unroll
+  for (int kk = 0; kk < BN / 16; ++kk)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) a_hi[kk][r] = a_lo[kk][r] = 0u;
+  float s[BN / 2];
+  // S = Q K^T of the key tile in stage st into s (issue only; the caller fences, commits and waits)
+  auto issue_s = [&](int st) {
+    const uint64_t kd = desc_stage(dk0, st, Cfg::K_BYTES);
+#pragma unroll
+    for (int ks = 0; ks < DQK / 16; ++ks) {
+      const int kb = ks * 32, bx = kb / SW, off = kb % SW;
+      wgmma_ss<BN, BF16, 0, 0>(s, desc_add(dq0, bx * Cfg::Q_BOX + off), desc_add(kd, bx * Cfg::K_BOX + off), ks > 0);
+    }
+  };
+  mbar_wait(&bars->q_full, 0);
+  mbar_wait(&bars->k_full[0], 0);
+  wgmma_fence();
+  issue_s(0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_regs(s);
+  release(kKey, 0, 0);
+  __syncwarp();
+  // Per tile i (s holds S_i): P_i -> A fragments; one MMA batch of O += P_i V_i and (kMerge) S_{i+1} = Q K_{i+1}^T; one wait;
+  // V_i and K_{i+1} are released.  O is never read inside the loop, so no MMA waits on the elementwise code of its own tile.
+  // The last tile (kLast) is peeled off the loop: it has no next tile, and it is the only one that can cross the sequence
+  // end (its key range ends at hi <= len), so the loop itself tests neither.
+  RingPos<NST> cur;  // ring stage and phase parity of tile i
+  auto tile = [&](int i, auto last_c) {
+    constexpr bool kLast = decltype(last_c)::value;
+    RingPos<NST> nx = cur;  // tile i + 1
+    nx.advance();
+    const int st = cur.st;
+    const int n0 = (t0 + i) * BN;
+    // P = silu(alpha S) * mask.  The mask case is chosen once per tile, outside the score loops, so that each loop is one
+    // basic block and ptxas can overlap the tanh of independent scores instead of waiting out each one in turn.
+    auto silu = [&](int n) {
+      const float x = s[n] * c_s, xp = kScaled ? x * c_p : x;
+      return __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
+    };
+    // a warp of padding rows only (delta) skips this stage: its A fragments keep the zeros they start with, so its P is 0
+    if (!rows_idle) {
+      if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
+#pragma unroll
+        for (int n = 0; n < BN / 2; ++n) s[n] = silu(n);
+      } else if (fast) {
+        // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limits of the thread's two rows hoisted
+        int lim[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
+#pragma unroll
+        for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+            const float pv = silu(nb * 4 + e);
+            s[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? pv : 0.f;
+          }
+      } else {
+#pragma unroll
+        for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+            const float pv = silu(nb * 4 + e);
+            s[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
+          }
+      }
+#pragma unroll
+      for (int kk = 0; kk < BN / 16; ++kk) {
+        const Operand<BF16> x0(s[8 * kk + 0], s[8 * kk + 1]), x1(s[8 * kk + 2], s[8 * kk + 3]);
+        const Operand<BF16> x2(s[8 * kk + 4], s[8 * kk + 5]), x3(s[8 * kk + 6], s[8 * kk + 7]);
+        a_hi[kk][0] = x0.hi; a_hi[kk][1] = x1.hi; a_hi[kk][2] = x2.hi; a_hi[kk][3] = x3.hi;
+        a_lo[kk][0] = x0.lo; a_lo[kk][1] = x1.lo; a_lo[kk][2] = x2.lo; a_lo[kk][3] = x3.lo;
+      }
+    }
+    mbar_wait(&bars->v_full[st], cur.ph);
+    // the last tile may cross the sequence end: its V rows >= len belong to the next sequence (P is 0 there, V may be NaN)
+    if (kLast && n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
+      zero_tile_rows<BN, SWV, Cfg::NBOX_V, kFwdThreads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, len - n0);
+      fence_proxy_async_smem();
+      named_bar_sync(kBarZeroRows, kFwdThreads);
+    }
+    if (kMerge && !kLast) mbar_wait(&bars->k_full[nx.st], nx.ph);
+    wgmma_fence();
+    const uint64_t vd = desc_stage(dv0, st, Cfg::V_BYTES);
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; ++kk) {
+      wgmma_rs<DV, BF16, 1>(o, a_hi[kk], desc_add(vd, kk * 16 * SWV), 1);
+      if constexpr (BF16) wgmma_rs<DV, BF16, 1>(o, a_lo[kk], desc_add(vd, kk * 16 * SWV), 1);
+    }
+    if (kMerge && !kLast) issue_s(nx.st);
+    wgmma_commit();
+    wgmma_wait<0>();  // an MMA batch never stays in flight across the elementwise code (ptxas would serialise them)
+    fence_regs(o);
+    fence_regs(a_hi);
+    fence_regs(a_lo);
+    fence_regs(s);
+    release(kVal, i, st);
+    if (!kMerge && !kLast) {
+      mbar_wait(&bars->k_full[nx.st], nx.ph);
+      wgmma_fence();
+      issue_s(nx.st);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+    }
+    if (!kLast) release(kKey, i + 1, nx.st);
+    __syncwarp();
+    cur = nx;
+  };
+  for (int i = 0; i < T - 1; ++i) tile(i, std::false_type{});
+  tile(T - 1, std::true_type{});
+
+  // ---------------- epilogue: O * 1/N -> global ----------------
+  if constexpr (kDelta) {  // row (local row lr) of out, or with more than one chunk the unscaled fp32 partial
+    const DeltaRows dr = delta_rows<Cfg::BM>(p);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int lr = wgi * 64 + w * 16 + g + hh * 8;
+      if (lr >= dr.rows) continue;
+      if (gridDim.z > 1) {
+        float* prow = p.part + ((dr.part_row + lr) * p.heads + h) * DV;
+#pragma unroll
+        for (int nb = 0; nb < DV / 8; ++nb)
+          *reinterpret_cast<float2*>(prow + nb * 8 + 2 * t4) = make_float2(o[nb * 4 + hh * 2], o[nb * 4 + hh * 2 + 1]);
+      } else {
+        uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (dr.out_row + lr) * p.o_row_stride + (long long)h * p.o_head_stride;
+#pragma unroll
+        for (int nb = 0; nb < DV / 8; ++nb) {
+          const float a = o[nb * 4 + hh * 2] * p.inv_n, c = o[nb * 4 + hh * 2 + 1] * p.inv_n;
+          *reinterpret_cast<uint32_t*>(orow + nb * 8 + 2 * t4) = BF16 ? pack_bf16x2(a, c) : pack_f16x2(a, c);
+        }
+      }
+    }
+    return;
+  }
+  const bool out_bf16 = BF16 || p.amax != nullptr;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int qi = q_base + hh * 8;
+    if (qi - m0 < mrows) {
+      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (row0 + qi) * p.o_row_stride + (long long)h * p.o_head_stride;
+#pragma unroll
+      for (int nb = 0; nb < DV / 8; ++nb) {
+        float a = o[nb * 4 + hh * 2] * p.inv_n, c = o[nb * 4 + hh * 2 + 1] * p.inv_n;
+        if (kScaled) a = scalbnf(a, e_out), c = scalbnf(c, e_out);
+        *reinterpret_cast<uint32_t*>(orow + nb * 8 + 2 * t4) = out_bf16 ? pack_bf16x2(a, c) : pack_f16x2(a, c);
+      }
+    }
+  }
+}
+
+
+// ------------------------------------------------------------------------------------------------
+// host
+// ------------------------------------------------------------------------------------------------
+// attn_wgmma_fwd.cu: the key chunks of a delta-q call (sizes only), and the reduction of their fp32 partials into out
+int delta_chunks(const hstu_attn_params& p);
+int launch_delta_reduce(bool bf16, const float* part, void* out, long long rows, int heads, int d, int chunks,
+                        long long o_row_stride, long long o_head_stride, float inv_n, cudaStream_t st);
+
+// kern: the kernel of this DQK / DV / BF16 / kDelta (an instance of attn_fwd_wgmma_body).  f16: the scaled fp16 copies of
+// bf16 inputs (the kernel is then the fp16 one), or null.  kDelta: a delta-q call, with the key chunks of delta_chunks and,
+// for more than one, the partials in the workspace and delta_reduce_kernel after the attention
+template <int DQK, int DV, bool BF16, bool kDelta>
+int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st, void (*kern)(FwdParams), const Fp16Operands* f16 = nullptr) {
+  using Cfg = FwdCfg<DQK, DV>;
+  FwdParams fp;
+  memset(&fp, 0, sizeof(fp));
+  const int chunks = kDelta ? delta_chunks(p) : 1;
+  if (chunks > 1) {
+    const size_t need = wgmma_delta_workspace_bytes(p);
+    if (p.workspace == nullptr || p.workspace_bytes < need) {
+      set_error("hstu_attn_fwd: delta_q workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
+      return HSTU_ERR_WORKSPACE;
+    }
+    fp.part = reinterpret_cast<float*>(p.workspace);
+  }
+  const long long q_rows = kDelta ? (long long)p.batch * p.delta_q_len : p.total_rows;
+  if (f16) {  // (dqk == dv == 32 only)
+    const long long crs = (long long)p.heads * DQK, chs = DQK;  // strides of the contiguous copies
+    if (int e = make_tmap_rows_heads(&fp.tmQ, f16->copy[0], p.total_rows, p.heads, DQK, crs, chs, Cfg::BOX_COLS, Cfg::BM)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmK, f16->copy[1], p.total_rows, p.heads, DQK, crs, chs, Cfg::BOX_COLS, Cfg::BN)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmV, f16->copy[2], p.total_rows, p.heads, DV, crs, chs, Cfg::BOX_COLS_V, Cfg::BN)) return e;
+    fp.amax = f16->amax;
+  } else {
+    if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, q_rows, p.heads, DQK, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BM)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, DQK, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
+    if (int e = make_tmap_rows_heads(&fp.tmV, p.v, p.total_rows, p.heads, DV, p.v_row_stride, p.v_head_stride, Cfg::BOX_COLS_V, Cfg::BN)) return e;
+  }
+  fp.heads = p.heads;
+  fp.seq_offsets = p.seq_offsets;
+  fp.num_targets = p.num_targets;
+  fp.out = p.out;
+  fp.o_row_stride = p.o_row_stride;
+  fp.o_head_stride = p.o_head_stride;
+  fp.offsets_i64 = p.offsets_are_i64;
+  fp.targets_i64 = p.num_targets_are_i64;
+  fp.max_seq_len = p.max_seq_len;
+  fp.win = p.max_attn_len;
+  fp.min_full = p.min_full_attn_seq_len;
+  fp.ctx = p.contextual_seq_len;
+  fp.alpha_half = 0.5f * p.alpha;
+  fp.inv_n = 1.0f / (float)p.max_seq_len;
+  fp.delta = p.delta_q_len;
+  HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+  const dim3 grid = kDelta ? dim3(p.batch * p.heads, (p.delta_q_len + Cfg::BM - 1) / Cfg::BM, chunks)
+                           : dim3((p.max_seq_len + Cfg::BM - 1) / Cfg::BM, p.heads, p.batch);
+  kern<<<grid, kFwdThreads, Cfg::SMEM_BYTES, st>>>(fp);
+  HSTU_CUDA_OK(cudaGetLastError());
+  if (chunks > 1) return launch_delta_reduce(BF16, fp.part, p.out, q_rows, p.heads, DV, chunks, p.o_row_stride, p.o_head_stride, fp.inv_n, st);
+  return 0;
+}
+
+}  // namespace hstu

@@ -17,6 +17,9 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd);
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
+// attn_wgmma_mixed_fwd.cu / attn_wgmma_mixed_bwd.cu: the same at dqk < dv (both in {32, 64, 128, 256})
+int attn_wgmma_fwd_mixed(const hstu_attn_params& p, cudaStream_t st);
+int attn_wgmma_bwd_mixed(const hstu_attn_params& p, cudaStream_t st);
 // the delta-q forward's fp32 partials of its key chunks (0 when one chunk suffices); sizes only
 size_t wgmma_delta_workspace_bytes(const hstu_attn_params& p);
 

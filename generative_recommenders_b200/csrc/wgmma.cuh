@@ -92,14 +92,23 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 template <int ROWS, int SW, int NBOX, int NTHREADS>
 __device__ __forceinline__ void zero_tile_rows(uint8_t* tile, int r0) {
   constexpr int kChunks = ROWS * SW / 16;  // 16-byte chunks per box, a fixed number per thread (few registers)
-  static_assert(kChunks % NTHREADS == 0, "whole chunks per thread");
+  if constexpr (kChunks % NTHREADS == 0) {
 #pragma unroll
-  for (int bx = 0; bx < NBOX; ++bx)
+    for (int bx = 0; bx < NBOX; ++bx)
 #pragma unroll
-    for (int k = 0; k < kChunks / NTHREADS; ++k) {
-      const int c = k * NTHREADS + (int)threadIdx.x;
-      if (c >= r0 * (SW / 16)) *reinterpret_cast<uint4*>(tile + bx * ROWS * SW + c * 16) = make_uint4(0u, 0u, 0u, 0u);
+      for (int k = 0; k < kChunks / NTHREADS; ++k) {
+        const int c = k * NTHREADS + (int)threadIdx.x;
+        if (c >= r0 * (SW / 16)) *reinterpret_cast<uint4*>(tile + bx * ROWS * SW + c * 16) = make_uint4(0u, 0u, 0u, 0u);
+      }
+  } else {  // boxes of fewer chunks than threads (narrow swizzle, few rows): NTHREADS / kChunks boxes per pass
+    static_assert(NTHREADS % kChunks == 0, "whole boxes per pass");
+    const int c = (int)threadIdx.x % kChunks;
+#pragma unroll
+    for (int bx0 = 0; bx0 < NBOX; bx0 += NTHREADS / kChunks) {
+      const int bx = bx0 + (int)threadIdx.x / kChunks;
+      if (bx < NBOX && c >= r0 * (SW / 16)) *reinterpret_cast<uint4*>(tile + bx * ROWS * SW + c * 16) = make_uint4(0u, 0u, 0u, 0u);
     }
+  }
 }
 constexpr int kBarZeroRows = 2;  // named barrier after zero_tile_rows (0 is __syncthreads, 1 the fused backward's dS barrier)
 

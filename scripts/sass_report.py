@@ -2,7 +2,7 @@
 
     python scripts/sass_report.py [--kernel SUBSTRING]
 
-Compiles attn_wgmma_fwd.cu, attn_wgmma_bwd.cu and attn_wgmma_fwd_e4m3.cu to sm_90a cubins with the flags of build.py plus `-Xptxas -v`, and prints
+Compiles the wgmma attention units (UNITS) to sm_90a cubins with the flags of build.py plus `-Xptxas -v`, and prints
 one JSON line per wgmma attention kernel: its registers, spill stores / loads (bytes), the ptxas notes and warnings it got
 (C7510 / C7512 / C7515: wgmma serialisation; C7519: a warpgroup.arrive ptxas inserted), and `tanh_per_block`, the most
 MUFU.TANH instructions in one basic block of its SASS (`cuobjdump -sass`).  A block ends at a branch and starts at a branch
@@ -25,7 +25,7 @@ import tempfile
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 CSRC = os.path.join(ROOT, "generative_recommenders_b200", "csrc")
-UNITS = ("attn_wgmma_fwd.cu", "attn_wgmma_bwd.cu", "attn_wgmma_fwd_e4m3.cu")
+UNITS = ("attn_wgmma_fwd.cu", "attn_wgmma_bwd.cu", "attn_wgmma_fwd_e4m3.cu", "attn_wgmma_mixed_fwd.cu", "attn_wgmma_mixed_bwd.cu")
 _CTRL = ("BRA", "BRX", "JMP", "JMX", "CALL", "RET", "EXIT", "BSSY")  # instructions that end a block or name a branch target
 
 
