@@ -6,18 +6,18 @@
 namespace hstu {
 
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_wgmma_kernel(const __grid_constant__ BwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, 1) attn_bwd_wgmma_kernel(const __grid_constant__ BwdParams p) {
   bwd_key_tile<D, D, BF16, true>(p);
 }
 
 // d = 32: two CTAs per SM (<= 128 registers per thread, 49 KB of shared memory); d = 256: one 128-column half per CTA
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dkdv_wgmma_kernel(const __grid_constant__ BwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, split_min_blocks(D)) attn_bwd_dkdv_wgmma_kernel(const __grid_constant__ BwdParams p) {
   bwd_key_tile<D, D, BF16, false>(p);
 }
 
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, split_min_blocks(D)) attn_bwd_dq_wgmma_kernel(const __grid_constant__ BwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, split_min_blocks(D)) attn_bwd_dq_wgmma_kernel(const __grid_constant__ BwdParams p) {
   bwd_dq_body<D, D, BF16>(p);
 }
 
@@ -104,7 +104,7 @@ static int launch_bwd_wgmma(const hstu_attn_params& p, cudaStream_t st, const Fp
     auto kern = attn_bwd_wgmma_kernel<D, BF16>;
     HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     dim3 grid((p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV, p.heads, p.batch);
-    kern<<<grid, kBwdThreads, Cfg::SMEM_BYTES, st>>>(bp);
+    kern<<<grid, kAttnThreads, Cfg::SMEM_BYTES, st>>>(bp);
     HSTU_CUDA_OK(cudaGetLastError());
     const long long nvec = p.total_rows * p.heads * (D / 8);
     long long blocks = (nvec + 255) / 256;

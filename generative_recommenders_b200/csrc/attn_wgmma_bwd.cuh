@@ -32,8 +32,8 @@
 //   attn_bwd_dkdv_wgmma_kernel  the kernel above without the dS buffers, the dS barrier and dQ: dK and dV only.
 //   attn_bwd_dq_wgmma_kernel    query-stationary, shaped like the forward: one CTA per (128-row query tile, head, sequence),
 //                               Q and dO resident, K and V streamed in 64-key tiles; it recomputes S = Q K^T and
-//                               dP = dO V^T, forms dS from one tanh and accumulates dQ += dS K in registers.  Its K / V ring
-//                               is refilled like the forward's, by the last warp to release a stage.
+//                               dP = dO V^T, forms dS from one tanh and accumulates dQ += dS K in registers.  Its prologue,
+//                               K / V ring and mask cases are the forward's (attn_wgmma_qtile.cuh).
 // Every dq / dk / dv element is then summed by one thread in a fixed order, so the result is bitwise reproducible.
 // At d = 32 recomputing S and dP costs two MMA units per score against the eight that the whole backward issues, while the
 // elementwise work per score is the same; at larger d the recomputed MMAs weigh more and the fused kernel stays the default.
@@ -53,6 +53,7 @@
 #include <type_traits>
 
 #include "attn_fp16_operands.cuh"
+#include "attn_wgmma_qtile.cuh"
 #include "common.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
@@ -60,22 +61,14 @@
 namespace hstu {
 using namespace wg;
 
-bool wgmma_fwd_supported(const hstu_attn_params& p);
-bool aligned_view(const void* ptr, long long row_stride, long long head_stride);
-
 struct alignas(64) BwdParams {
   CUtensorMap tmQ, tmK, tmV, tmDO;
-  const void* seq_offsets;
-  const void* num_targets;
+  SeqArgs seq;
   void* dk;
   void* dv;
   float* dq_acc;  // [L, H, DQK] fp32, zero-initialised (fused kernel)
   void* dq;       // attn_bwd_dq_wgmma_kernel
   long long dk_row_stride, dk_head_stride, dv_row_stride, dv_head_stride, dq_row_stride, dq_head_stride;
-  int offsets_i64, targets_i64;
-  int max_seq_len, heads;
-  int win, min_full, ctx;
-  float alpha_half;
   float dv_scale;  // 1 / N
   float dk_scale;  // alpha / (2 N): dS^T holds 2 dS N / alpha
   const uint32_t* amax;  // fp16 kernels on scaled copies of bf16 inputs: [B, H, 4] amax bits (attn_fp16_operands.cuh); else null
@@ -87,10 +80,10 @@ struct BwdScales {
   float c_s = 0.f, c_p = 1.f, c_d = 1.f;  // alpha / 2 * 2^-(e_q + e_k), 2^e_p, 2^(e_s - e_v - e_o)
   int e_dv = 0, e_dk = 0, e_dq = 0;       // epilogue exponents: -(e_p + e_o), -(e_s + e_q), -(e_s + e_k)
   __device__ __forceinline__ BwdScales(const BwdParams& p, int b, int h, int d) {
-    c_s = p.alpha_half;
+    c_s = p.seq.alpha_half;
     if (p.amax == nullptr) return;
-    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, 2.f * p.alpha_half, d);
-    c_s = ldexpf(p.alpha_half, -(ex.q + ex.k));
+    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.seq.heads + h) * kAmaxSlots, 2.f * p.seq.alpha_half, d);
+    c_s = ldexpf(p.seq.alpha_half, -(ex.q + ex.k));
     c_p = pow2f(ex.p);
     c_d = pow2f(ex.s - ex.v - ex.o);
     e_dv = -(ex.p + ex.o);
@@ -106,7 +99,6 @@ constexpr int kSmemPerSm = 232448;  // dynamic shared memory one CTA may use on 
 // registers per thread (and 64 + 64 fp32 accumulators of d = 256 would take 256); there two CTAs per key tile take one half
 // of the dK and of the dV columns each
 __host__ __device__ constexpr int dkdv_slices(int dv) { return dv == 256 ? 2 : 1; }
-__host__ __device__ constexpr int swizzle_bytes(int cols) { return cols * 2 >= 128 ? 128 : cols * 2; }
 __host__ __device__ constexpr int imax(int a, int b) { return a > b ? a : b; }
 
 // FUSED_DQ: the key-tile kernel also computes dQ (dS buffers in shared memory); without it the layout ends after the ring,
@@ -142,7 +134,6 @@ struct BwdCfg {
   static_assert(SMEM_BYTES * (FUSED_DQ ? 1 : split_min_blocks(DV)) <= kSmemPerSm, "shared memory budget");
   static_assert(STAGES <= 4, "BwdBars holds four stages");
 };
-constexpr int kBwdThreads = 256;
 
 struct BwdBars {
   uint64_t kv_full;
@@ -170,18 +161,18 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   const int b = blockIdx.z, h = blockIdx.y;
   const int n0 = (blockIdx.x / NSL) * Cfg::BKV;
   const int ck0 = (blockIdx.x % NSL) * DNK, cv0 = (blockIdx.x % NSL) * DNV;
-  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
-  int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
-  if (len > p.max_seq_len) {  // rows past max_seq_len get zero gradients
+  const long long row0 = load_index(p.seq.seq_offsets, p.seq.offsets_i64, b);
+  int len = (int)(load_index(p.seq.seq_offsets, p.seq.offsets_i64, b + 1) - row0);
+  if (len > p.seq.max_seq_len) {  // rows past max_seq_len get zero gradients
     if (blockIdx.x == 0) {
-      zero_rows(p.dk, 2, p.dk_row_stride, (long long)h * p.dk_head_stride, DQK, row0 + p.max_seq_len, row0 + len);
-      zero_rows(p.dv, 2, p.dv_row_stride, (long long)h * p.dv_head_stride, DV, row0 + p.max_seq_len, row0 + len);
+      zero_rows(p.dk, 2, p.dk_row_stride, (long long)h * p.dk_head_stride, DQK, row0 + p.seq.max_seq_len, row0 + len);
+      zero_rows(p.dv, 2, p.dv_row_stride, (long long)h * p.dv_head_stride, DV, row0 + p.seq.max_seq_len, row0 + len);
     }
-    len = p.max_seq_len;
+    len = p.seq.max_seq_len;
   }
   if (n0 >= len) return;
-  const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
-  const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
+  const int n_tgt = p.seq.num_targets ? (int)load_index(p.seq.num_targets, p.seq.targets_i64, b) : -1;
+  const SeqMask msk = make_seq_mask(len, n_tgt, p.seq.win, p.seq.min_full, p.seq.ctx);
   const int nrows = min(Cfg::BKV, len - n0);
   QTiles qt;
   {
@@ -192,8 +183,7 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     qt.T = qt.A + max(0, (hi + BQ - 1) / BQ - qt.first);
   }
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = dyn_smem_1k();
   BwdBars* bars = reinterpret_cast<BwdBars*>(smem + Cfg::OFF_BAR);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
@@ -265,11 +255,8 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
 
   mbar_wait(&bars->kv_full, 0);
   // K rows >= len of a key tile that crosses the sequence end are B of dQ = dS K (dS is 0 there, K may be NaN)
-  if (FUSED_DQ && n0 + Cfg::BKV > len) {  // CTA-uniform; K is loaded once
-    zero_tile_rows<Cfg::BKV, SW, Cfg::NBOX, kBwdThreads>(smem + Cfg::OFF_K, len - n0);
-    fence_proxy_async_smem();
-    named_bar_sync(kBarZeroRows, kBwdThreads);
-  }
+  if (FUSED_DQ && n0 + Cfg::BKV > len)  // CTA-uniform; K is loaded once
+    zero_tile_rows_sync<Cfg::BKV, SW, Cfg::NBOX, kAttnThreads>(smem + Cfg::OFF_K, len - n0);
   for (int j = 0; j < qt.T; ++j) {
     const int st = j % NST;
     const uint32_t ph = (j / NST) & 1;
@@ -279,10 +266,8 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     // tile that crosses the sequence end is the last one of the key tile (hi <= len, ctx_hi <= len), so its stage is not
     // refilled after the zeroing.
     if (q0 + BQ > len) {  // CTA-uniform
-      zero_tile_rows<BQ, SWQ, Cfg::NBOX_Q, kBwdThreads>(smem + Cfg::OFF_Q + st * Cfg::Q_BYTES, len - q0);
-      zero_tile_rows<BQ, SWV, Cfg::NBOX_V, kBwdThreads>(smem + Cfg::OFF_DO + st * Cfg::DO_BYTES, len - q0);
-      fence_proxy_async_smem();
-      named_bar_sync(kBarZeroRows, kBwdThreads);
+      zero_tile_rows<BQ, SWQ, Cfg::NBOX_Q, kAttnThreads>(smem + Cfg::OFF_Q + st * Cfg::Q_BYTES, len - q0);
+      zero_tile_rows_sync<BQ, SWV, Cfg::NBOX_V, kAttnThreads>(smem + Cfg::OFF_DO + st * Cfg::DO_BYTES, len - q0);
     }
     float s[BQ / 2], dp[BQ / 2];
     wgmma_fence();
@@ -307,7 +292,7 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     // The mask case is chosen once per tile, outside the score loops, so that ptxas can overlap the tanh of independent
     // scores (as in the forward).  `v`: the pair is valid.
     auto score = [&](int n, bool v) {
-      const float x = s[n] * (kScaled ? sc.c_s : p.alpha_half), xp = kScaled ? x * sc.c_p : x;
+      const float x = s[n] * (kScaled ? sc.c_s : p.seq.alpha_half), xp = kScaled ? x * sc.c_p : x;
       const float t = tanh_approx(x);
       const float g2 = __fmaf_rn(x, __fmaf_rn(-t, t, 1.f), t);
       const float pv = __fmaf_rn(xp, t, xp);
@@ -406,7 +391,7 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
     fence_regs(df_hi);
     fence_regs(df_lo);
     // Q_j and dO_j are no longer read by this warp; the last of the eight warps to say so refills the stage
-    if (lane == 0 && j + NST < qt.T && release_is_last<kBwdThreads / 32>(&bars->qd_free[st])) load_qd(j + NST);
+    if (lane == 0 && j + NST < qt.T && release_is_last<kAttnThreads / 32>(&bars->qd_free[st])) load_qd(j + NST);
     __syncwarp();
     if constexpr (!FUSED_DQ) continue;
     // dS^T -> shared memory buffer j & 1: element (kv r, q c) of a [128][64] 16-bit box with 128-byte swizzle
@@ -442,7 +427,7 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
         for (int hh = 0; hh < 2; ++hh) {
           const int qi = qrow + hh * 8;
           if (qi < len) {
-            float* dst = p.dq_acc + ((row0 + qi) * p.heads + h) * DQK + pass * Cfg::DQN + 2 * t4;
+            float* dst = p.dq_acc + ((row0 + qi) * p.seq.heads + h) * DQK + pass * Cfg::DQN + 2 * t4;
 #pragma unroll
             for (int nb = 0; nb < Cfg::DQN / 8; ++nb)
               atomicAdd(reinterpret_cast<float2*>(dst + nb * 8), make_float2(dq[nb * 4 + hh * 2], dq[nb * 4 + hh * 2 + 1]));
@@ -502,13 +487,8 @@ struct DqCfg {
   static_assert(SMEM_BYTES * split_min_blocks(DV) <= kSmemPerSm, "shared memory budget of split_min_blocks(dv) CTAs per SM");
 };
 
-struct DqBars {
-  uint64_t qd_full;
-  uint64_t k_full[3], v_full[3];
-  uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
-};
-
-// One CTA per (128-row query tile, head, sequence), heavy (late) tiles first; the forward's schedule, tile ranges and ring.
+// One CTA per (128-row query tile, head, sequence), heavy (late) tiles first; the forward's schedule, tile ranges and ring
+// (attn_wgmma_qtile.cuh).
 // Per 64-key tile each warpgroup runs S = Q K^T and dP = dO V^T (A and B K-major), releases V, forms
 // 2 dS N / alpha = dP (1 + g2) * mask from one tanh, and runs dQ += dS K (A from registers, K read MN-major), then releases K.
 // Q, K and dQ are DQK wide, dO and V DV wide.
@@ -519,74 +499,27 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
   constexpr bool kScaled = !BF16 && DQK == 32 && DV == 32;  // also runs bf16 inputs on scaled fp16 copies
   const int b = blockIdx.z, h = blockIdx.y;
   const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
-  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
-  int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
-  if (len > p.max_seq_len) {  // rows past max_seq_len get zero gradients
-    if (blockIdx.x == 0) zero_rows(p.dq, 2, p.dq_row_stride, (long long)h * p.dq_head_stride, DQK, row0 + p.max_seq_len, row0 + len);
-    len = p.max_seq_len;
-  }
-  if (m0 >= len) return;
-  const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
-  const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
-  const int mrows = min(Cfg::BM, len - m0);
-  int lo, hi;
-  kv_range_for_q_rows(msk, m0, m0 + mrows, &lo, &hi);
-  const int t0 = lo / BN;
-  const int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
+  QTileSeq qs;  // (rows past max_seq_len get zero gradients)
+  if (!qtile_prologue<Cfg::BM, BN>(p.seq, b, h, m0, p.dq, p.dq_row_stride, p.dq_head_stride, DQK, &qs)) return;
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  DqBars* bars = reinterpret_cast<DqBars*>(smem + Cfg::OFF_BAR);
+  uint8_t* smem = dyn_smem_1k();
+  // V of tile i is released once the warp's S / dP MMAs have completed, K once its dQ MMAs have
+  KvRing<Cfg> ring{smem, &p.tmK, &p.tmV, h, qs.row0, qs.t0, qs.T};
+  ring.init();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(&bars->qd_full, 1);
-    for (int i = 0; i < NST; ++i) {
-      mbar_init(&bars->k_full[i], 1);
-      mbar_init(&bars->v_full[i], 1);
-      bars->k_free[i] = bars->v_free[i] = 0u;
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  // TMA issue of key tile i into its K (kKey) or V (kVal) stage st
-  constexpr std::false_type kKey{};
-  constexpr std::true_type kVal{};
-  auto load = [&](auto val_c, int i, int st) {
-    constexpr bool kIsV = decltype(val_c)::value;
-    constexpr int bytes = kIsV ? Cfg::V_BYTES : Cfg::K_BYTES, box = kIsV ? Cfg::V_BOX : Cfg::K_BOX;
-    constexpr int nbox = kIsV ? Cfg::NBOX_V : Cfg::NBOX, cols = kIsV ? Cfg::BOX_COLS_V : Cfg::BOX_COLS;
-    uint64_t* full = kIsV ? bars->v_full : bars->k_full;
-    mbar_arrive_expect_tx(&full[st], bytes);
-#pragma unroll
-    for (int bx = 0; bx < nbox; ++bx)
-      tma_load_3d(smem + (kIsV ? Cfg::OFF_V : Cfg::OFF_K) + st * bytes + bx * box, kIsV ? &p.tmV : &p.tmK, &full[st], bx * cols, h,
-                  (int)(row0 + (long long)(t0 + i) * BN));
-  };
-  // Thread 0 loads Q, dO and the first STAGES key tiles.  Afterwards each warp releases the V stage of tile i once its S / dP
-  // MMAs have completed and the K stage once its dQ MMAs have, and the warp whose release is the last of the eight loads tile
-  // i + STAGES into the stage (the forward's protocol).
-  // (st: the stage of tile i, i % NST)
-  auto release = [&](auto val_c, int i, int st) {
-    uint32_t* ctr = decltype(val_c)::value ? bars->v_free : bars->k_free;
-    if (lane == 0 && i + NST < T && release_is_last<kBwdThreads / 32>(&ctr[st])) load(val_c, i + NST, st);
-  };
   if (tid == 0) {
     prefetch_tensormap(&p.tmQ);
     prefetch_tensormap(&p.tmK);
     prefetch_tensormap(&p.tmV);
     prefetch_tensormap(&p.tmDO);
-    mbar_arrive_expect_tx(&bars->qd_full, Cfg::Q_BYTES + Cfg::DO_BYTES);
+    mbar_arrive_expect_tx(&ring.bars->q_full, Cfg::Q_BYTES + Cfg::DO_BYTES);
 #pragma unroll
     for (int bx = 0; bx < imax(Cfg::NBOX, Cfg::NBOX_V); ++bx) {
-      if (bx < Cfg::NBOX) tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->qd_full, bx * Cfg::BOX_COLS, h, (int)(row0 + m0));
+      if (bx < Cfg::NBOX) tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &ring.bars->q_full, bx * Cfg::BOX_COLS, h, (int)(qs.row0 + m0));
       if (bx < Cfg::NBOX_V)
-        tma_load_3d(smem + Cfg::OFF_DO + bx * Cfg::DO_BOX, &p.tmDO, &bars->qd_full, bx * Cfg::BOX_COLS_V, h, (int)(row0 + m0));
+        tma_load_3d(smem + Cfg::OFF_DO + bx * Cfg::DO_BOX, &p.tmDO, &ring.bars->q_full, bx * Cfg::BOX_COLS_V, h, (int)(qs.row0 + m0));
     }
-    for (int i = 0; i < min(T, NST); ++i) {
-      load(kKey, i, i);
-      load(kVal, i, i);
-    }
+    ring.fill();
   }
   __syncwarp();
 
@@ -599,8 +532,8 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
   const uint64_t dk0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_K), 0));
   const uint64_t dv0 = desc_pin(desc_kmajor<SWV>(smem_u32(smem + Cfg::OFF_V), 0));
   const uint64_t dkn0 = desc_pin(desc_mnmajor<SW>(smem_u32(smem + Cfg::OFF_K), 0, Cfg::K_BOX));
-  const bool fast = msk.fast != 0;
-  const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
+  const bool fast = qs.msk.fast != 0;
+  const int full_lim = full_valid_limit(qs.msk, m0);
 
   const BwdScales sc(p, b, h, DQK);
   float dq[DQK / 2];
@@ -613,23 +546,20 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
     for (int r = 0; r < 4; ++r) a_hi[kk][r] = a_lo[kk][r] = 0u;
   // One wait per MMA batch: S and dP of tile i + 1 in the batch of dQ += dS_i K_i would hold S, dP, dQ and both dS fragment
   // sets at once, which does not fit in 128 registers with bf16 inputs (ptxas spills and serialises the MMAs).
-  mbar_wait(&bars->qd_full, 0);
+  mbar_wait(&ring.bars->q_full, 0);
   // The last tile (kLast) is peeled off the loop: it is the only one that can cross the sequence end (its key range ends at
   // hi <= len), so the loop itself does not test for it.
   RingPos<NST> cur;  // ring stage and phase parity of tile i
   auto tile = [&](int i, auto last_c) {
     constexpr bool kLast = decltype(last_c)::value;
     const int st = cur.st;
-    const int n0 = (t0 + i) * BN;
+    const int n0 = (qs.t0 + i) * BN;
     float s[BN / 2], dp[BN / 2];
-    mbar_wait(&bars->k_full[st], cur.ph);
-    mbar_wait(&bars->v_full[st], cur.ph);
+    ring.wait(kKey, st, cur.ph);
+    ring.wait(kVal, st, cur.ph);
     // the last key tile may cross the sequence end: its K rows >= len are B of dQ += dS K (dS is 0 there, K may be NaN)
-    if (kLast && n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
-      zero_tile_rows<BN, SW, Cfg::NBOX, kBwdThreads>(smem + Cfg::OFF_K + st * Cfg::K_BYTES, len - n0);
-      fence_proxy_async_smem();
-      named_bar_sync(kBarZeroRows, kBwdThreads);
-    }
+    if (kLast && n0 + BN > qs.len)  // CTA-uniform; the last tile, so its stage is not refilled
+      zero_tile_rows_sync<BN, SW, Cfg::NBOX, kAttnThreads>(smem + Cfg::OFF_K + st * Cfg::K_BYTES, qs.len - n0);
     wgmma_fence();
     const uint64_t kd = desc_stage(dk0, st, Cfg::K_BYTES), vd = desc_stage(dv0, st, Cfg::V_BYTES);
 #pragma unroll
@@ -646,11 +576,10 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
     wgmma_wait<0>();
     fence_regs(s);
     fence_regs(dp);
-    release(kVal, i, st);
+    ring.release(kVal, i, st);
     __syncwarp();
 
-    // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2.  The mask case is chosen once per
-    // tile, outside the score loops, so that ptxas can overlap the tanh of independent scores (as in the forward).
+    // 2 dS N / alpha = dP (1 + g2), g2 = t + h (1 - t^2), t = tanh h, h = alpha s / 2
     auto dscore = [&](int n) {
       const float x = s[n] * sc.c_s;
       const float t = tanh_approx(x);
@@ -659,32 +588,7 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
       if (kScaled) dsv *= sc.c_d;
       return dsv;
     };
-    if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
-#pragma unroll
-      for (int n = 0; n < BN / 2; ++n) dp[n] = dscore(n);
-    } else if (fast) {
-      // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limits of the thread's two rows hoisted
-      int lim[2];
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
-#pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float dsv = dscore(nb * 4 + e);
-          dp[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? dsv : 0.f;
-        }
-    } else {
-#pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float dsv = dscore(nb * 4 + e);
-          dp[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? dsv : 0.f;
-        }
-    }
+    mask_scores<BN>(qs.msk, fast, full_lim, qs.len, q_base, n0, t4, dp, dscore);
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk) {
 #pragma unroll
@@ -706,19 +610,19 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
     fence_regs(dq);
     fence_regs(a_hi);
     fence_regs(a_lo);
-    release(kKey, i, st);
+    ring.release(kKey, i, st);
     __syncwarp();
     cur.advance();
   };
-  for (int i = 0; i < T - 1; ++i) tile(i, std::false_type{});
-  tile(T - 1, std::true_type{});
+  for (int i = 0; i < qs.T - 1; ++i) tile(i, std::false_type{});
+  tile(qs.T - 1, std::true_type{});
 
   // ---------------- epilogue: dQ * alpha / (2N) -> global ----------------
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int qi = q_base + hh * 8;
-    if (qi - m0 < mrows) {
-      uint16_t* qrow = reinterpret_cast<uint16_t*>(p.dq) + (row0 + qi) * p.dq_row_stride + (long long)h * p.dq_head_stride;
+    if (qi - m0 < qs.mrows) {
+      uint16_t* qrow = reinterpret_cast<uint16_t*>(p.dq) + (qs.row0 + qi) * p.dq_row_stride + (long long)h * p.dq_head_stride;
 #pragma unroll
       for (int nb = 0; nb < DQK / 8; ++nb) {
         float a = dq[nb * 4 + hh * 2] * p.dk_scale, c = dq[nb * 4 + hh * 2 + 1] * p.dk_scale;
@@ -751,8 +655,7 @@ inline BwdParams bwd_params(const hstu_attn_params& p, const Fp16Operands* f16) 
   BwdParams bp;
   memset(&bp, 0, sizeof(bp));
   if (f16) bp.amax = f16->amax;
-  bp.seq_offsets = p.seq_offsets;
-  bp.num_targets = p.num_targets;
+  bp.seq = seq_args(p);
   bp.dk = p.dk;
   bp.dv = p.dv_out;
   bp.dq_acc = reinterpret_cast<float*>(p.workspace);
@@ -763,14 +666,6 @@ inline BwdParams bwd_params(const hstu_attn_params& p, const Fp16Operands* f16) 
   bp.dv_head_stride = p.dv_head_stride;
   bp.dq_row_stride = p.dq_row_stride;
   bp.dq_head_stride = p.dq_head_stride;
-  bp.offsets_i64 = p.offsets_are_i64;
-  bp.targets_i64 = p.num_targets_are_i64;
-  bp.max_seq_len = p.max_seq_len;
-  bp.heads = p.heads;
-  bp.win = p.max_attn_len;
-  bp.min_full = p.min_full_attn_seq_len;
-  bp.ctx = p.contextual_seq_len;
-  bp.alpha_half = 0.5f * p.alpha;
   bp.dv_scale = 1.0f / (float)p.max_seq_len;
   bp.dk_scale = 0.5f * p.alpha / (float)p.max_seq_len;
   return bp;
@@ -793,7 +688,7 @@ int launch_bwd_split(const hstu_attn_params& p, cudaStream_t st, void (*kdkdv)(B
   HSTU_CUDA_OK(cudaFuncSetAttribute(kdkdv, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   // the column slices of one key tile are adjacent CTAs (they read the same K, V and query tiles)
   const int key_ctas = (p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV * Cfg::NSL;
-  kdkdv<<<dim3(key_ctas, p.heads, p.batch), kBwdThreads, Cfg::SMEM_BYTES, st>>>(bp);
+  kdkdv<<<dim3(key_ctas, p.heads, p.batch), kAttnThreads, Cfg::SMEM_BYTES, st>>>(bp);
   HSTU_CUDA_OK(cudaGetLastError());
   // the dQ kernel tiles 128 query rows and DqCfg::BN key rows
   using QC = DqCfg<DQK, DV>;
@@ -802,7 +697,7 @@ int launch_bwd_split(const hstu_attn_params& p, cudaStream_t st, void (*kdkdv)(B
   if (int e = make_tmap_rows_heads(&bp.tmV, o.src[2], p.total_rows, p.heads, d[2], o.rs[2], o.hs[2], QC::BOX_COLS_V, QC::BN)) return e;
   if (int e = make_tmap_rows_heads(&bp.tmDO, o.src[3], p.total_rows, p.heads, d[3], o.rs[3], o.hs[3], QC::BOX_COLS_V, QC::BM)) return e;
   HSTU_CUDA_OK(cudaFuncSetAttribute(kdq, cudaFuncAttributeMaxDynamicSharedMemorySize, QC::SMEM_BYTES));
-  kdq<<<dim3((p.max_seq_len + QC::BM - 1) / QC::BM, p.heads, p.batch), kBwdThreads, QC::SMEM_BYTES, st>>>(bp);
+  kdq<<<dim3((p.max_seq_len + QC::BM - 1) / QC::BM, p.heads, p.batch), kAttnThreads, QC::SMEM_BYTES, st>>>(bp);
   HSTU_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -6,11 +6,11 @@
 namespace hstu {
 
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_kernel(const __grid_constant__ FwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, kFwdMinBlocks<D>) attn_fwd_wgmma_kernel(const __grid_constant__ FwdParams p) {
   attn_fwd_wgmma_body<D, D, BF16, false>(p);
 }
 template <int D, bool BF16>
-__global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<D>) attn_fwd_delta_wgmma_kernel(const __grid_constant__ FwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, kFwdMinBlocks<D>) attn_fwd_delta_wgmma_kernel(const __grid_constant__ FwdParams p) {
   attn_fwd_wgmma_body<D, D, BF16, true>(p);
 }
 

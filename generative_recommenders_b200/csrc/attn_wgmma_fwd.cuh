@@ -11,11 +11,9 @@
 // Key tiles of 64 rows keep a thread at <= 128 registers for d <= 64, so two CTAs share an SM there.
 // Each warpgroup waits for its own MMAs; the two warpgroups overlap each other's tensor-core and elementwise phases.  With
 // d <= 64, O += P_i V_i and S_{i+1} = Q K_{i+1}^T are one MMA batch with one wait per tile (O is never read in the loop).
-// Thread 0 issues the first TMA loads: Q, then the K and V tiles through a ring of STAGES buffers each.  Each warp releases a
-// stage once its MMAs that read it have completed, and the warp whose release is the last of the eight issues the refill
-// (release_is_last, wgmma.cuh), so no thread ever waits for a free stage and neither warpgroup holds the other back.  No
-// separate producer warp: the 64 x d fp32 O accumulator (d = 256: 128 registers per thread) needs the register budget of a
-// 256-thread block.
+// Q is loaded once; the K and V tiles go through the ring of attn_wgmma_qtile.cuh (STAGES buffers each, refilled by the last
+// warp to release a stage, no producer warp: the 64 x d fp32 O accumulator, 128 registers per thread at d = 256, needs the
+// register budget of a 256-thread block).
 // P is a 16-bit MMA operand of the same format as V (wgmma takes one format for A and B): fp16 for fp16 inputs, and for
 // bf16 inputs a hi + lo pair of bf16 operands multiplied twice (wgmma.cuh, Operand), so that its rounding stays well inside
 // the 1e-3 parity budget.  bf16 inputs at d = 32 instead run the fp16 kernel on exactly scaled fp16 copies of q, k, v with
@@ -41,6 +39,7 @@
 #include <type_traits>
 
 #include "attn_fp16_operands.cuh"
+#include "attn_wgmma_qtile.cuh"
 #include "common.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
@@ -50,17 +49,11 @@ using namespace wg;
 
 struct alignas(64) FwdParams {
   CUtensorMap tmQ, tmK, tmV;
-  const void* seq_offsets;
-  const void* num_targets;
+  SeqArgs seq;
   void* out;
   long long o_row_stride, o_head_stride;
-  int offsets_i64, targets_i64;
-  int max_seq_len;
-  int win, min_full, ctx;
-  float alpha_half;  // alpha / 2
-  float inv_n;       // 1 / max_seq_len
+  float inv_n;  // 1 / max_seq_len
   const uint32_t* amax;  // fp16 kernel on scaled copies of bf16 inputs: [B, H, 4] amax bits (attn_fp16_operands.cuh); else null
-  int heads;
   // delta-q only (kDelta): query rows per sequence, and with gridDim.z > 1 key chunks the fp32 partials [chunks, B * delta, H, DV]
   int delta;
   float* part;
@@ -70,8 +63,7 @@ template <int DQK, int DV = DQK>
 struct FwdCfg {
   static constexpr int BM = 128;                     // query rows per CTA (two warpgroups of 64)
   static constexpr int BN = 64;                      // key rows per tile
-  static constexpr int SW = (DQK * 2 >= 128) ? 128 : DQK * 2;  // swizzle width (bytes) of the Q / K boxes
-  static constexpr int SWV = (DV * 2 >= 128) ? 128 : DV * 2;   // and of the V boxes
+  static constexpr int SW = swizzle_bytes(DQK), SWV = swizzle_bytes(DV);  // swizzle width (bytes) of the Q / K boxes, of the V boxes
   static constexpr int BOX_COLS = SW / 2;
   static constexpr int BOX_COLS_V = SWV / 2;
   static constexpr int Q_BOX = BM * SW;
@@ -92,15 +84,8 @@ struct FwdCfg {
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
   static_assert(DQK <= DV, "dqk > dv has no instantiation");
 };
-constexpr int kFwdThreads = 256;
 // dv <= 64: two CTAs per SM (<= 128 registers per thread; the O accumulator is dv / 2 of them)
 template <int DV> constexpr int kFwdMinBlocks = (DV <= 64) ? 2 : 1;
-
-struct FwdBars {
-  uint64_t q_full;
-  uint64_t k_full[3], v_full[3];
-  uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
-};
 
 // Delta-q: the output row (of q / out, and of the partials of chunk blockIdx.z) of local query row 0 of the CTA, and the CTA's
 // valid query rows.  Recomputed from the grid where needed, so that nothing extra stays live through the key loop.
@@ -111,8 +96,8 @@ struct DeltaRows {
 template <int BM>
 __device__ __forceinline__ DeltaRows delta_rows(const FwdParams& p) {
   const int m0 = (int)blockIdx.y * BM;
-  const long long r = (long long)(blockIdx.x / p.heads) * p.delta + m0;
-  return {r, (long long)blockIdx.z * (gridDim.x / p.heads) * p.delta + r, min(BM, p.delta - m0)};
+  const long long r = (long long)(blockIdx.x / p.seq.heads) * p.delta + m0;
+  return {r, (long long)blockIdx.z * (gridDim.x / p.seq.heads) * p.delta + r, min(BM, p.delta - m0)};
 }
 
 // kDelta: the delta-q geometry and key chunks described at the top (grid (B * H, query tiles, chunks)); otherwise the full
@@ -125,115 +110,68 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
   // dv <= 64: P V of tile i and S of tile i + 1 form one MMA batch with one wait (both fit in 128 registers); larger dv waits
   // for each batch separately, since the O accumulator leaves no room for S next to the P fragments
   constexpr bool kMerge = DV <= 64;
-  const int b = kDelta ? (int)blockIdx.x / p.heads : (int)blockIdx.z, h = kDelta ? (int)blockIdx.x % p.heads : (int)blockIdx.y;
+  const int b = kDelta ? (int)blockIdx.x / p.seq.heads : (int)blockIdx.z, h = kDelta ? (int)blockIdx.x % p.seq.heads : (int)blockIdx.y;
   const int m0 = kDelta ? (int)blockIdx.y * Cfg::BM : (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;  // first query row of the CTA
-  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
-  int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
-  if (!kDelta && len > p.max_seq_len) {  // rows past max_seq_len are ignored on the way in and zero on the way out
-    if (blockIdx.x == 0) zero_rows(p.out, 2, p.o_row_stride, (long long)h * p.o_head_stride, DV, row0 + p.max_seq_len, row0 + len);
-    len = p.max_seq_len;
+  QTileSeq qs;
+  if constexpr (kDelta) {  // query row i at position len - delta + i; the whole sequence, unclipped
+    seq_rows(p.seq, b, &qs);
+  } else if (!qtile_rows(p.seq, b, h, m0, p.out, p.o_row_stride, p.o_head_stride, DV, &qs)) {
+    return;
   }
-  if (!kDelta && m0 >= len) return;
-  const int p0 = kDelta ? len - p.delta + m0 : m0;  // sequence position of query row m0 (delta: the last delta rows)
-  const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
-  const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
-  const int mrows = min(Cfg::BM, (kDelta ? p.delta : len) - m0);
-  int lo, hi;
-  kv_range_for_q_rows(msk, p0, p0 + mrows, &lo, &hi);
-  int t0 = lo / BN;
-  int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
+  const int p0 = kDelta ? qs.len - p.delta + m0 : m0;  // sequence position of query row m0 (delta: the last delta rows)
+  key_tiles<Cfg::BM, BN>(p.seq, b, p0, (kDelta ? p.delta : qs.len) - m0, &qs);
   if constexpr (kDelta) {
     // chunk blockIdx.z of gridDim.z even shares of whole tiles; an empty share (or no key at all) writes zeros, so that
     // every partial the reduction reads is defined
-    const int per = (T + (int)gridDim.z - 1) / (int)gridDim.z;
-    t0 += (int)blockIdx.z * per;
-    T = min(per, T - (int)blockIdx.z * per);
-    if (T <= 0) {
+    const int per = (qs.T + (int)gridDim.z - 1) / (int)gridDim.z;
+    qs.t0 += (int)blockIdx.z * per;
+    qs.T = min(per, qs.T - (int)blockIdx.z * per);
+    if (qs.T <= 0) {
       const DeltaRows dr = delta_rows<Cfg::BM>(p);
-      for (int idx = threadIdx.x; idx < dr.rows * DV; idx += kFwdThreads) {
-        if (gridDim.z > 1) p.part[((dr.part_row + idx / DV) * p.heads + h) * DV + idx % DV] = 0.f;
+      for (int idx = threadIdx.x; idx < dr.rows * DV; idx += kAttnThreads) {
+        if (gridDim.z > 1) p.part[((dr.part_row + idx / DV) * p.seq.heads + h) * DV + idx % DV] = 0.f;
         else reinterpret_cast<uint16_t*>(p.out)[(dr.out_row + idx / DV) * p.o_row_stride + (long long)h * p.o_head_stride + idx % DV] = 0;
       }
       return;
     }
   }
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  FwdBars* bars = reinterpret_cast<FwdBars*>(smem + Cfg::OFF_BAR);
+  uint8_t* smem = dyn_smem_1k();
+  KvRing<Cfg> ring{smem, &p.tmK, &p.tmV, h, qs.row0, qs.t0, qs.T};
+  ring.init();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(&bars->q_full, 1);
-    for (int i = 0; i < NST; ++i) {
-      mbar_init(&bars->k_full[i], 1);
-      mbar_init(&bars->v_full[i], 1);
-      bars->k_free[i] = bars->v_free[i] = 0u;
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  // TMA issue of key tile i into its K (kKey) or V (kVal) stage st
-  constexpr std::false_type kKey{};
-  constexpr std::true_type kVal{};
-  auto load = [&](auto val_c, int i, int st) {
-    constexpr bool kIsV = decltype(val_c)::value;
-    constexpr int bytes = kIsV ? Cfg::V_BYTES : Cfg::K_BYTES, box = kIsV ? Cfg::V_BOX : Cfg::K_BOX;
-    constexpr int nbox = kIsV ? Cfg::NBOX_V : Cfg::NBOX, cols = kIsV ? Cfg::BOX_COLS_V : Cfg::BOX_COLS;
-    uint64_t* full = kIsV ? bars->v_full : bars->k_full;
-    mbar_arrive_expect_tx(&full[st], bytes);
-#pragma unroll
-    for (int bx = 0; bx < nbox; ++bx)
-      tma_load_3d(smem + (kIsV ? Cfg::OFF_V : Cfg::OFF_K) + st * bytes + bx * box, kIsV ? &p.tmV : &p.tmK, &full[st], bx * cols, h,
-                  (int)(row0 + (long long)(t0 + i) * BN));
-  };
-  // Thread 0 loads Q and the first STAGES key tiles.  Afterwards nobody waits for a free stage: each warp releases the K (V)
-  // stage of tile i once its MMAs that read it have completed, and the warp whose release is the last of the eight issues
-  // the load of tile i + STAGES into it, so neither warpgroup holds the other back.
-  // (st: the stage of tile i, i % NST)
-  auto release = [&](auto val_c, int i, int st) {
-    uint32_t* ctr = decltype(val_c)::value ? bars->v_free : bars->k_free;
-    if (lane == 0 && i + NST < T && release_is_last<kFwdThreads / 32>(&ctr[st])) load(val_c, i + NST, st);
-  };
   if (tid == 0) {
     prefetch_tensormap(&p.tmQ);
     prefetch_tensormap(&p.tmK);
     prefetch_tensormap(&p.tmV);
-    mbar_arrive_expect_tx(&bars->q_full, Cfg::Q_BYTES);
+    mbar_arrive_expect_tx(&ring.bars->q_full, Cfg::Q_BYTES);
 #pragma unroll
     for (int bx = 0; bx < Cfg::NBOX; ++bx)
-      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::BOX_COLS, h,
-                  kDelta ? b * p.delta + m0 : (int)(row0 + m0));
-    for (int i = 0; i < min(T, NST); ++i) {
-      load(kKey, i, i);
-      load(kVal, i, i);
-    }
+      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &ring.bars->q_full, bx * Cfg::BOX_COLS, h,
+                  kDelta ? b * p.delta + m0 : (int)(qs.row0 + m0));
+    ring.fill();
   }
   __syncwarp();
 
   // (delta: the plain index; the descriptors held in registers through its loop would spill at d = 64 with bf16 inputs)
   const int wgi = kDelta ? warp >> 2 : warpgroup_index(), w = warp & 3, g = lane >> 2, t4 = lane & 3;
   if constexpr (kDelta) {
-    if (wgi * 64 >= mrows) {
+    if (wgi * 64 >= qs.mrows) {
       // a warpgroup of padding rows only: no MMA, no tanh, no output.  It still releases every stage use, once that use has
       // landed (its full barrier), so that its releases cannot run ahead into the next use of the stage and complete a
       // release while another warp still reads it; and it helps zero the V rows past the sequence end (CTA-wide barrier)
-      mbar_wait(&bars->k_full[0], 0);
-      release(kKey, 0, 0);
-      for (int i = 0; i < T; ++i) {
+      ring.wait(kKey, 0, 0);
+      ring.release(kKey, 0, 0);
+      for (int i = 0; i < qs.T; ++i) {
         const int st = i % NST;
-        const bool next = i + 1 < T;
-        const int n0 = (t0 + i) * BN;
-        mbar_wait(&bars->v_full[st], (i / NST) & 1);
-        if (n0 + BN > len) {
-          zero_tile_rows<BN, SWV, Cfg::NBOX_V, kFwdThreads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, len - n0);
-          fence_proxy_async_smem();
-          named_bar_sync(kBarZeroRows, kFwdThreads);
-        }
-        if (next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+        const bool next = i + 1 < qs.T;
+        const int n0 = (qs.t0 + i) * BN;
+        ring.wait(kVal, st, (i / NST) & 1);
+        if (n0 + BN > qs.len) zero_tile_rows_sync<BN, SWV, Cfg::NBOX_V, kAttnThreads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, qs.len - n0);
+        if (next) ring.wait(kKey, (i + 1) % NST, ((i + 1) / NST) & 1);
         __syncwarp();
-        release(kVal, i, st);
-        if (next) release(kKey, i + 1, (i + 1) % NST);
+        ring.release(kVal, i, st);
+        if (next) ring.release(kKey, i + 1, (i + 1) % NST);
         __syncwarp();
       }
       return;
@@ -241,21 +179,21 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
   }
   const int q_base = p0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
   // delta: a warp whose 16 rows all lie past delta skips the elementwise stage (warp-uniform)
-  const bool rows_idle = kDelta && wgi * 64 + w * 16 >= mrows;
+  const bool rows_idle = kDelta && wgi * 64 + w * 16 >= qs.mrows;
   // wgmma descriptors, built once: Q of the warpgroup, and K (K-major) and V (MN-major) of ring stage 0; everything else is
   // a constant step from them (desc_add), and all three are warp-uniform
   const uint64_t dq0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SW, 0));
   const uint64_t dk0 = desc_pin(desc_kmajor<SW>(smem_u32(smem + Cfg::OFF_K), 0));
   const uint64_t dv0 = desc_pin(desc_mnmajor<SWV>(smem_u32(smem + Cfg::OFF_V), 0, Cfg::V_BOX));
-  const bool fast = msk.fast != 0;
-  const int full_lim = fast ? min(p0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
+  const bool fast = qs.msk.fast != 0;
+  const int full_lim = full_valid_limit(qs.msk, p0);
   // scaled fp16 operands: S holds 2^(e_q + e_k) S, P is formed as 2^e_p P and O holds 2^(e_p + e_v) O
   constexpr bool kScaled = !kDelta && !BF16 && DQK == 32 && DV == 32;  // the only instantiation that runs bf16 inputs on fp16 copies
-  float c_s = p.alpha_half, c_p = 1.f;
+  float c_s = p.seq.alpha_half, c_p = 1.f;
   int e_out = 0;
   if (kScaled && p.amax != nullptr) {
-    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.heads + h) * kAmaxSlots, 2.f * p.alpha_half, DQK);
-    c_s = ldexpf(p.alpha_half, -(ex.q + ex.k));
+    const OperandExps ex = operand_exps(p.amax + ((long long)b * p.seq.heads + h) * kAmaxSlots, 2.f * p.seq.alpha_half, DQK);
+    c_s = ldexpf(p.seq.alpha_half, -(ex.q + ex.k));
     c_p = pow2f(ex.p);
     e_out = -(ex.p + ex.v);
   }
@@ -278,14 +216,14 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
       wgmma_ss<BN, BF16, 0, 0>(s, desc_add(dq0, bx * Cfg::Q_BOX + off), desc_add(kd, bx * Cfg::K_BOX + off), ks > 0);
     }
   };
-  mbar_wait(&bars->q_full, 0);
-  mbar_wait(&bars->k_full[0], 0);
+  mbar_wait(&ring.bars->q_full, 0);
+  ring.wait(kKey, 0, 0);
   wgmma_fence();
   issue_s(0);
   wgmma_commit();
   wgmma_wait<0>();
   fence_regs(s);
-  release(kKey, 0, 0);
+  ring.release(kKey, 0, 0);
   __syncwarp();
   // Per tile i (s holds S_i): P_i -> A fragments; one MMA batch of O += P_i V_i and (kMerge) S_{i+1} = Q K_{i+1}^T; one wait;
   // V_i and K_{i+1} are released.  O is never read inside the loop, so no MMA waits on the elementwise code of its own tile.
@@ -297,41 +235,15 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
     RingPos<NST> nx = cur;  // tile i + 1
     nx.advance();
     const int st = cur.st;
-    const int n0 = (t0 + i) * BN;
-    // P = silu(alpha S) * mask.  The mask case is chosen once per tile, outside the score loops, so that each loop is one
-    // basic block and ptxas can overlap the tanh of independent scores instead of waiting out each one in turn.
+    const int n0 = (qs.t0 + i) * BN;
+    // P = silu(alpha S) * mask
     auto silu = [&](int n) {
       const float x = s[n] * c_s, xp = kScaled ? x * c_p : x;
       return __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
     };
     // a warp of padding rows only (delta) skips this stage: its A fragments keep the zeros they start with, so its P is 0
     if (!rows_idle) {
-      if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
-#pragma unroll
-        for (int n = 0; n < BN / 2; ++n) s[n] = silu(n);
-      } else if (fast) {
-        // mask_valid of the fast mask, kj < min(qi, max_id) || kj == qi, with the limits of the thread's two rows hoisted
-        int lim[2];
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
-#pragma unroll
-        for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-            const float pv = silu(nb * 4 + e);
-            s[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? pv : 0.f;
-          }
-      } else {
-#pragma unroll
-        for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-            const float pv = silu(nb * 4 + e);
-            s[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
-          }
-      }
+      mask_scores<BN>(qs.msk, fast, full_lim, qs.len, q_base, n0, t4, s, silu);
 #pragma unroll
       for (int kk = 0; kk < BN / 16; ++kk) {
         const Operand<BF16> x0(s[8 * kk + 0], s[8 * kk + 1]), x1(s[8 * kk + 2], s[8 * kk + 3]);
@@ -340,14 +252,11 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
         a_lo[kk][0] = x0.lo; a_lo[kk][1] = x1.lo; a_lo[kk][2] = x2.lo; a_lo[kk][3] = x3.lo;
       }
     }
-    mbar_wait(&bars->v_full[st], cur.ph);
+    ring.wait(kVal, st, cur.ph);
     // the last tile may cross the sequence end: its V rows >= len belong to the next sequence (P is 0 there, V may be NaN)
-    if (kLast && n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
-      zero_tile_rows<BN, SWV, Cfg::NBOX_V, kFwdThreads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, len - n0);
-      fence_proxy_async_smem();
-      named_bar_sync(kBarZeroRows, kFwdThreads);
-    }
-    if (kMerge && !kLast) mbar_wait(&bars->k_full[nx.st], nx.ph);
+    if (kLast && n0 + BN > qs.len)  // CTA-uniform; the last tile, so its stage is not refilled
+      zero_tile_rows_sync<BN, SWV, Cfg::NBOX_V, kAttnThreads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, qs.len - n0);
+    if (kMerge && !kLast) ring.wait(kKey, nx.st, nx.ph);
     wgmma_fence();
     const uint64_t vd = desc_stage(dv0, st, Cfg::V_BYTES);
 #pragma unroll
@@ -362,21 +271,21 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
     fence_regs(a_hi);
     fence_regs(a_lo);
     fence_regs(s);
-    release(kVal, i, st);
+    ring.release(kVal, i, st);
     if (!kMerge && !kLast) {
-      mbar_wait(&bars->k_full[nx.st], nx.ph);
+      ring.wait(kKey, nx.st, nx.ph);
       wgmma_fence();
       issue_s(nx.st);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(s);
     }
-    if (!kLast) release(kKey, i + 1, nx.st);
+    if (!kLast) ring.release(kKey, i + 1, nx.st);
     __syncwarp();
     cur = nx;
   };
-  for (int i = 0; i < T - 1; ++i) tile(i, std::false_type{});
-  tile(T - 1, std::true_type{});
+  for (int i = 0; i < qs.T - 1; ++i) tile(i, std::false_type{});
+  tile(qs.T - 1, std::true_type{});
 
   // ---------------- epilogue: O * 1/N -> global ----------------
   if constexpr (kDelta) {  // row (local row lr) of out, or with more than one chunk the unscaled fp32 partial
@@ -386,7 +295,7 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
       const int lr = wgi * 64 + w * 16 + g + hh * 8;
       if (lr >= dr.rows) continue;
       if (gridDim.z > 1) {
-        float* prow = p.part + ((dr.part_row + lr) * p.heads + h) * DV;
+        float* prow = p.part + ((dr.part_row + lr) * p.seq.heads + h) * DV;
 #pragma unroll
         for (int nb = 0; nb < DV / 8; ++nb)
           *reinterpret_cast<float2*>(prow + nb * 8 + 2 * t4) = make_float2(o[nb * 4 + hh * 2], o[nb * 4 + hh * 2 + 1]);
@@ -405,8 +314,8 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int qi = q_base + hh * 8;
-    if (qi - m0 < mrows) {
-      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (row0 + qi) * p.o_row_stride + (long long)h * p.o_head_stride;
+    if (qi - m0 < qs.mrows) {
+      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (qs.row0 + qi) * p.o_row_stride + (long long)h * p.o_head_stride;
 #pragma unroll
       for (int nb = 0; nb < DV / 8; ++nb) {
         float a = o[nb * 4 + hh * 2] * p.inv_n, c = o[nb * 4 + hh * 2 + 1] * p.inv_n;
@@ -455,25 +364,16 @@ int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st, void (*kern)(Fw
     if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, DQK, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
     if (int e = make_tmap_rows_heads(&fp.tmV, p.v, p.total_rows, p.heads, DV, p.v_row_stride, p.v_head_stride, Cfg::BOX_COLS_V, Cfg::BN)) return e;
   }
-  fp.heads = p.heads;
-  fp.seq_offsets = p.seq_offsets;
-  fp.num_targets = p.num_targets;
+  fp.seq = seq_args(p);
   fp.out = p.out;
   fp.o_row_stride = p.o_row_stride;
   fp.o_head_stride = p.o_head_stride;
-  fp.offsets_i64 = p.offsets_are_i64;
-  fp.targets_i64 = p.num_targets_are_i64;
-  fp.max_seq_len = p.max_seq_len;
-  fp.win = p.max_attn_len;
-  fp.min_full = p.min_full_attn_seq_len;
-  fp.ctx = p.contextual_seq_len;
-  fp.alpha_half = 0.5f * p.alpha;
   fp.inv_n = 1.0f / (float)p.max_seq_len;
   fp.delta = p.delta_q_len;
   HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   const dim3 grid = kDelta ? dim3(p.batch * p.heads, (p.delta_q_len + Cfg::BM - 1) / Cfg::BM, chunks)
                            : dim3((p.max_seq_len + Cfg::BM - 1) / Cfg::BM, p.heads, p.batch);
-  kern<<<grid, kFwdThreads, Cfg::SMEM_BYTES, st>>>(fp);
+  kern<<<grid, kAttnThreads, Cfg::SMEM_BYTES, st>>>(fp);
   HSTU_CUDA_OK(cudaGetLastError());
   if (chunks > 1) return launch_delta_reduce(BF16, fp.part, p.out, q_rows, p.heads, DV, chunks, p.o_row_stride, p.o_head_stride, fp.inv_n, st);
   return 0;

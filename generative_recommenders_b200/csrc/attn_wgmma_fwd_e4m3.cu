@@ -28,8 +28,6 @@
 namespace hstu {
 using namespace wg;
 
-bool aligned_view(const void* ptr, long long row_stride, long long head_stride);  // attn_wgmma_fwd.cu
-
 struct alignas(64) E4m3FwdParams {
   CUtensorMap tmQ, tmK, tmV;  // Q, K: the e4m3 inputs (bytes); V: the fp16 copy of v
   const void* seq_offsets;

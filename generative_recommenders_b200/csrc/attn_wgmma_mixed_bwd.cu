@@ -12,11 +12,11 @@
 namespace hstu {
 
 template <int DQK, int DV, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, split_min_blocks(DV)) attn_bwd_dkdv_mixed_wgmma_kernel(const __grid_constant__ BwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, split_min_blocks(DV)) attn_bwd_dkdv_mixed_wgmma_kernel(const __grid_constant__ BwdParams p) {
   bwd_key_tile<DQK, DV, BF16, false>(p);
 }
 template <int DQK, int DV, bool BF16>
-__global__ void __launch_bounds__(kBwdThreads, split_min_blocks(DV)) attn_bwd_dq_mixed_wgmma_kernel(const __grid_constant__ BwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, split_min_blocks(DV)) attn_bwd_dq_mixed_wgmma_kernel(const __grid_constant__ BwdParams p) {
   bwd_dq_body<DQK, DV, BF16>(p);
 }
 

@@ -8,11 +8,11 @@
 namespace hstu {
 
 template <int DQK, int DV, bool BF16>
-__global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<DV>) attn_fwd_mixed_wgmma_kernel(const __grid_constant__ FwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, kFwdMinBlocks<DV>) attn_fwd_mixed_wgmma_kernel(const __grid_constant__ FwdParams p) {
   attn_fwd_wgmma_body<DQK, DV, BF16, false>(p);
 }
 template <int DQK, int DV, bool BF16>
-__global__ void __launch_bounds__(kFwdThreads, kFwdMinBlocks<DV>) attn_fwd_delta_mixed_wgmma_kernel(const __grid_constant__ FwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, kFwdMinBlocks<DV>) attn_fwd_delta_mixed_wgmma_kernel(const __grid_constant__ FwdParams p) {
   attn_fwd_wgmma_body<DQK, DV, BF16, true>(p);
 }
 

@@ -20,6 +20,10 @@ int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
 // attn_wgmma_mixed_fwd.cu / attn_wgmma_mixed_bwd.cu: the same at dqk < dv (both in {32, 64, 128, 256})
 int attn_wgmma_fwd_mixed(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd_mixed(const hstu_attn_params& p, cudaStream_t st);
+// attn_wgmma_fwd.cu: a 16-bit view the kernels take (16-byte base, row / head strides of whole 16-byte units), and whether
+// the wgmma forward takes the call (dtype, dims, alignment of q, k, v, out; sm_90)
+bool aligned_view(const void* ptr, long long row_stride, long long head_stride);
+bool wgmma_fwd_supported(const hstu_attn_params& p);
 // the delta-q forward's fp32 partials of its key chunks (0 when one chunk suffices); sizes only
 size_t wgmma_delta_workspace_bytes(const hstu_attn_params& p);
 

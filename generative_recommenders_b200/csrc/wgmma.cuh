@@ -13,6 +13,11 @@ namespace hstu {
 namespace wg {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// The CTA's dynamic shared memory from its first 1024-byte boundary (the alignment of a 128-byte swizzle atom)
+__device__ __forceinline__ uint8_t* dyn_smem_1k() {
+  extern __shared__ uint8_t smem_raw[];
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+}
 
 #ifndef HSTU_WAIT_LIMIT_CLK
 #define HSTU_WAIT_LIMIT_CLK 4000000000ll  // bounded wait (~2 s): a protocol bug traps instead of hanging the GPU
@@ -87,8 +92,8 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 // Zeroes rows [r0, ROWS) of a TMA-loaded tile of NBOX swizzled boxes of [ROWS][SW bytes] (a row is one contiguous SW-byte line
 // of its box whatever the swizzle), so that rows a box dragged in past a sequence end cannot reach an MMA: a zero in the
 // other factor does not neutralise them, 0 * NaN = NaN.  Called by all NTHREADS threads of the CTA after the tile's full
-// barrier; the caller then issues fence_proxy_async_smem() and a CTA-wide named barrier, so that no warpgroup's wgmma reads
-// the tile before every row is zero, and makes sure the stage is not refilled while the zeros are still needed.
+// barrier, and followed by the fence and CTA-wide barrier of zero_tile_rows_sync (on the last tile zeroed).  The caller makes
+// sure the stage is not refilled while the zeros are still needed.
 template <int ROWS, int SW, int NBOX, int NTHREADS>
 __device__ __forceinline__ void zero_tile_rows(uint8_t* tile, int r0) {
   constexpr int kChunks = ROWS * SW / 16;  // 16-byte chunks per box, a fixed number per thread (few registers)
@@ -111,6 +116,13 @@ __device__ __forceinline__ void zero_tile_rows(uint8_t* tile, int r0) {
   }
 }
 constexpr int kBarZeroRows = 2;  // named barrier after zero_tile_rows (0 is __syncthreads, 1 the fused backward's dS barrier)
+// zero_tile_rows, made visible to the MMAs (async proxy) of both warpgroups: none reads the tile before every row is zero
+template <int ROWS, int SW, int NBOX, int NTHREADS>
+__device__ __forceinline__ void zero_tile_rows_sync(uint8_t* tile, int r0) {
+  zero_tile_rows<ROWS, SW, NBOX, NTHREADS>(tile, r0);
+  fence_proxy_async_smem();
+  named_bar_sync(kBarZeroRows, NTHREADS);
+}
 
 // ---------------------------------------------------------------------------------------------
 // TMA loads (tile mode) into shared memory, completion on an mbarrier
@@ -130,9 +142,9 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 // ---------------------------------------------------------------------------------------------
 // 64-bit shared-memory matrix descriptor (sm_90): start address, leading / stride byte offsets (16-byte units), swizzle mode
 // in bits 62-63 (1 = 128B, 2 = 64B, 3 = 32B).  Tiles are aligned to their swizzle atom, so the base-offset field stays 0.
-__host__ __device__ constexpr int swizzle_mode(int swizzle_bytes) {
-  return swizzle_bytes == 128 ? 1 : swizzle_bytes == 64 ? 2 : swizzle_bytes == 32 ? 3 : 0;
-}
+__host__ __device__ constexpr int swizzle_mode(int sw) { return sw == 128 ? 1 : sw == 64 ? 2 : sw == 32 ? 3 : 0; }
+// Swizzle width (bytes) of the TMA boxes of an operand whose rows are `cols` elements: the whole row up to 128 bytes
+__host__ __device__ constexpr int swizzle_bytes(int cols, int elem_bytes = 2) { return cols * elem_bytes >= 128 ? 128 : cols * elem_bytes; }
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, int mode) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
