@@ -1,288 +1,14 @@
 // Jagged HSTU attention forward on float8 e4m3 q, k, v with per (sequence, head) descales, bf16 output, on the Hopper
-// warpgroup tensor cores.  dqk == dv in {32, 64, 128, 256} (DESIGN.md 3.5).
-//
-//   out = attention(q * qd[b, h], k * kd[b, h], v * vd[b, h])
-//
-// The structure is the bf16 / fp16 forward's (attn_wgmma_fwd.cu): one CTA per (128-row query tile, head, sequence), heavy
-// tiles first; two warpgroups of 64 query rows; 64-key tiles through a ring of STAGES K and V buffers, refilled by the warp
-// whose release is the last of the eight (release_is_last, the same protocol); tile-uniform mask cases; with d <= 64, O +=
-// P_i V_i and S_{i+1} = Q K_{i+1}^T form one MMA batch with one wait.  What differs:
-//   S = Q K^T  on fp8 tensor cores (wgmma m64n64k32 e4m3, both operands K-major).  Q and K are TMA-staged as bytes; a row
-//              of d e4m3 values has the layout of a 16-bit row of d / 2, so the K-major descriptors apply with 32-byte k
-//              steps.  Swizzle: 32 B at d = 32, 64 B at d = 64, 128-byte boxes at d >= 128.
-//   P          = silu(alpha qd kd S) * mask, formed as one fp16 operand P' = P 2^p (e4m3_p_exp: a bound from the e4m3
-//              range, no amax pass).
-//   O += P' V  16-bit, on the exact fp16 copy of v that a pre-pass writes into the workspace (attn_fp16_operands.cu): fp16
-//              P keeps the operand rounding inside the bf16 parity bound, which an e4m3 P would not (DESIGN.md 3.5).
-//   epilogue   O * (1/N) vd 2^-p -> bf16.
-// Rows of the fp16 v copy past a sequence end are the next sequence's rows (or rows at positions >= max_seq_len, which the
-// pre-pass never writes), so the V stage of the tile that crosses the end is zeroed past it (zero_tile_rows), as in the
-// bf16 forward.  Scales are per (sequence, head): a NaN or Inf descale or input value changes no other (sequence, head).
-#include <string.h>
-
-#include "attn_fp16_operands.cuh"
-#include "common.cuh"
-#include "internal.h"
-#include "wgmma.cuh"
+// warpgroup tensor cores, at dqk == dv in {32, 64, 128, 256}; the host checks and routing of every fp8 forward.  The kernel
+// body, its design and its launcher are in attn_wgmma_fwd_e4m3.cuh; the dqk < dv instantiations are in
+// attn_wgmma_mixed_fwd_e4m3.cu (DESIGN.md 3.5).
+#include "attn_wgmma_fwd_e4m3.cuh"
 
 namespace hstu {
-using namespace wg;
-
-struct alignas(64) E4m3FwdParams {
-  CUtensorMap tmQ, tmK, tmV;  // Q, K: the e4m3 inputs (bytes); V: the fp16 copy of v
-  const void* seq_offsets;
-  const void* num_targets;
-  void* out;  // bf16
-  long long o_row_stride, o_head_stride;
-  const float* descale[3];  // q, k, v: [B, H] fp32, or null (= 1)
-  long long ds_batch[3], ds_head[3];
-  int offsets_i64, targets_i64;
-  int max_seq_len;
-  int win, min_full, ctx;
-  float alpha_half;  // alpha / 2
-  float alpha;
-  float inv_n;       // 1 / max_seq_len
-};
-
-template <int D>
-struct E4m3FwdCfg {
-  static constexpr int BM = 128;  // query rows per CTA (two warpgroups of 64)
-  static constexpr int BN = 64;   // key rows per tile
-  static constexpr int SWK = D >= 128 ? 128 : D;         // swizzle (bytes) of the e4m3 Q / K boxes: one byte per element
-  static constexpr int SWV = 2 * D >= 128 ? 128 : 2 * D;  // of the fp16 V boxes
-  static constexpr int QK_BOX_COLS = SWK, V_BOX_COLS = SWV / 2;
-  static constexpr int NBOX_QK = D / QK_BOX_COLS, NBOX_V = D / V_BOX_COLS;
-  static constexpr int Q_BOX = BM * SWK, K_BOX = BN * SWK, V_BOX = BN * SWV;
-  static constexpr int Q_BYTES = BM * D, K_BYTES = BN * D, V_BYTES = BN * D * 2;
-  static constexpr int STAGES = 3;
-  static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = OFF_Q + Q_BYTES;
-  static constexpr int OFF_V = OFF_K + STAGES * K_BYTES;
-  static constexpr int OFF_BAR = OFF_V + STAGES * V_BYTES;
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;  // + barriers + alignment slack
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-  static_assert(OFF_K % 1024 == 0 && OFF_V % 1024 == 0 && K_BYTES % 256 == 0 && V_BYTES % 1024 == 0, "swizzle atom alignment");
-};
-constexpr int kE4m3Threads = 256;
-template <int D> constexpr int kE4m3MinBlocks = (D <= 64) ? 2 : 1;  // d <= 64: two CTAs per SM (<= 128 registers per thread)
-
-struct E4m3Bars {
-  uint64_t q_full;
-  uint64_t k_full[3], v_full[3];
-  uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
-};
-
-__device__ __forceinline__ float load_descale(const float* d, long long bs, long long hs, int b, int h) {
-  return d ? d[(long long)b * bs + (long long)h * hs] : 1.f;
-}
 
 template <int D>
 __global__ void __launch_bounds__(kE4m3Threads, kE4m3MinBlocks<D>) attn_fwd_e4m3_wgmma_kernel(const __grid_constant__ E4m3FwdParams p) {
-  using Cfg = E4m3FwdCfg<D>;
-  constexpr int SWK = Cfg::SWK, SWV = Cfg::SWV, BN = Cfg::BN, NST = Cfg::STAGES;
-  constexpr bool kMerge = D <= 64;  // as in the bf16 forward: S_{i+1} and P_i V_i in one batch where the registers allow
-  const int b = blockIdx.z, h = blockIdx.y;
-  const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
-  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
-  int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
-  if (len > p.max_seq_len) {  // rows past max_seq_len are ignored on the way in and zero on the way out
-    if (blockIdx.x == 0) zero_rows(p.out, 2, p.o_row_stride, (long long)h * p.o_head_stride, D, row0 + p.max_seq_len, row0 + len);
-    len = p.max_seq_len;
-  }
-  if (m0 >= len) return;
-  const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
-  const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
-  const int mrows = min(Cfg::BM, len - m0);
-  int lo, hi;
-  kv_range_for_q_rows(msk, m0, m0 + mrows, &lo, &hi);
-  const int t0 = lo / BN;
-  const int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  E4m3Bars* bars = reinterpret_cast<E4m3Bars*>(smem + Cfg::OFF_BAR);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(&bars->q_full, 1);
-    for (int i = 0; i < NST; ++i) {
-      mbar_init(&bars->k_full[i], 1);
-      mbar_init(&bars->v_full[i], 1);
-      bars->k_free[i] = bars->v_free[i] = 0u;
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  const int key_row0 = (int)(row0 + (long long)t0 * BN);
-  auto load_k = [&](int i) {
-    const int st = i % NST;
-    mbar_arrive_expect_tx(&bars->k_full[st], Cfg::K_BYTES);
-#pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX_QK; ++bx)
-      tma_load_3d(smem + Cfg::OFF_K + st * Cfg::K_BYTES + bx * Cfg::K_BOX, &p.tmK, &bars->k_full[st], bx * Cfg::QK_BOX_COLS, h,
-                  key_row0 + i * BN);
-  };
-  auto load_v = [&](int i) {
-    const int st = i % NST;
-    mbar_arrive_expect_tx(&bars->v_full[st], Cfg::V_BYTES);
-#pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX_V; ++bx)
-      tma_load_3d(smem + Cfg::OFF_V + st * Cfg::V_BYTES + bx * Cfg::V_BOX, &p.tmV, &bars->v_full[st], bx * Cfg::V_BOX_COLS, h,
-                  key_row0 + i * BN);
-  };
-  // the ring protocol of the bf16 forward: each warp releases the K (V) stage of tile i once its MMAs that read it have
-  // completed, and the warp whose release is the last of the eight loads tile i + STAGES into it
-  auto release_k = [&](int i) {
-    if (lane == 0 && i + NST < T && release_is_last<kE4m3Threads / 32>(&bars->k_free[i % NST])) load_k(i + NST);
-  };
-  auto release_v = [&](int i) {
-    if (lane == 0 && i + NST < T && release_is_last<kE4m3Threads / 32>(&bars->v_free[i % NST])) load_v(i + NST);
-  };
-  if (tid == 0) {
-    prefetch_tensormap(&p.tmQ);
-    prefetch_tensormap(&p.tmK);
-    prefetch_tensormap(&p.tmV);
-    mbar_arrive_expect_tx(&bars->q_full, Cfg::Q_BYTES);
-#pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX_QK; ++bx)
-      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::QK_BOX_COLS, h, (int)(row0 + m0));
-    for (int i = 0; i < min(T, NST); ++i) {
-      load_k(i);
-      load_v(i);
-    }
-  }
-  __syncwarp();
-
-  const int wgi = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
-  const int q_base = m0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
-  const uint32_t sq = smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SWK;
-  const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
-  const bool fast = msk.fast != 0;
-  const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
-  // scales of this (sequence, head): S holds S / (qd kd), P is formed as 2^e_p P, O holds 2^e_p O / vd.
-  const float qd = load_descale(p.descale[0], p.ds_batch[0], p.ds_head[0], b, h);
-  const float kd = load_descale(p.descale[1], p.ds_batch[1], p.ds_head[1], b, h);
-  const float vd = load_descale(p.descale[2], p.ds_batch[2], p.ds_head[2], b, h);
-  // The scalars are built from the frexp mantissas (in [0.5, 1)) and exponents of the factors, so that small but legal
-  // descales lose no precision in fp32 subnormals: c_sp = alpha/2 qd kd 2^e_p forms P' and is a normal number (m 2^(-4 - log2 d)
-  // unless e_p is clamped); c_s = alpha/2 qd kd is only the tanh argument's scale, and where it underflows |x| < 2^-100, so
-  // tanh x is nothing next to the 1 of 1 + tanh x.  The output scale (1/N) vd 2^-e_p is applied as the normal c_o = (1/N) m_v
-  // and an exact power of two.  Zero, Inf and NaN factors propagate as before (frexpf keeps them).
-  const int e_p = e4m3_p_exp(p.alpha, qd, kd, D);
-  int ea, eq, ek, ev;
-  const float m_s = frexpf(p.alpha_half, &ea) * frexpf(qd, &eq) * frexpf(kd, &ek);
-  const float c_s = scalbnf(m_s, ea + eq + ek), c_sp = scalbnf(m_s, ea + eq + ek + e_p);
-  const float c_o = p.inv_n * frexpf(vd, &ev);
-  const int e_o = ev - e_p;
-
-  float o[D / 2];
-#pragma unroll
-  for (int e = 0; e < D / 2; ++e) o[e] = 0.f;
-  uint32_t a[BN / 16][4];
-#pragma unroll
-  for (int kk = 0; kk < BN / 16; ++kk)
-#pragma unroll
-    for (int r = 0; r < 4; ++r) a[kk][r] = 0u;
-  float s[BN / 2];
-  // S = Q K_i^T into s (issue only; the caller fences, commits and waits)
-  auto issue_s = [&](int i) {
-    const uint32_t kst = sk + (i % NST) * Cfg::K_BYTES;
-#pragma unroll
-    for (int ks = 0; ks < D / 32; ++ks) {
-      const int kb = ks * 32, bx = kb / SWK, off = kb % SWK;
-      wgmma_ss_64_e4m3(s, desc_kmajor<SWK>(sq + bx * Cfg::Q_BOX, off), desc_kmajor<SWK>(kst + bx * Cfg::K_BOX, off), ks > 0);
-    }
-  };
-  mbar_wait(&bars->q_full, 0);
-  mbar_wait(&bars->k_full[0], 0);
-  wgmma_fence();
-  issue_s(0);
-  wgmma_commit();
-  wgmma_wait<0>();
-  fence_regs(s);
-  release_k(0);
-  __syncwarp();
-  for (int i = 0; i < T; ++i) {
-    const int st = i % NST;
-    const bool next = i + 1 < T;
-    const int n0 = (t0 + i) * BN;
-    // P' = 2^e_p silu(alpha S) * mask; the mask case is chosen once per tile, so each score loop is one basic block
-    auto silu = [&](int n) {
-      const float x = s[n] * c_s, xp = s[n] * c_sp;
-      return __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
-    };
-    if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
-#pragma unroll
-      for (int n = 0; n < BN / 2; ++n) s[n] = silu(n);
-    } else if (fast) {
-      int lim[2];
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
-#pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float pv = silu(nb * 4 + e);
-          s[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? pv : 0.f;
-        }
-    } else {
-#pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float pv = silu(nb * 4 + e);
-          s[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
-        }
-    }
-#pragma unroll
-    for (int kk = 0; kk < BN / 16; ++kk)
-#pragma unroll
-      for (int r = 0; r < 4; ++r) a[kk][r] = pack_f16x2_sat(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
-    mbar_wait(&bars->v_full[st], (i / NST) & 1);
-    // the last tile may cross the sequence end: its V rows >= len belong to the next sequence (P is 0 there, V may be NaN)
-    if (n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
-      zero_tile_rows<BN, SWV, Cfg::NBOX_V, kE4m3Threads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, len - n0);
-      fence_proxy_async_smem();
-      named_bar_sync(kBarZeroRows, kE4m3Threads);
-    }
-    if (kMerge && next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < BN / 16; ++kk)
-      wgmma_rs<D, false, 1>(o, a[kk], desc_mnmajor<SWV>(sv + st * Cfg::V_BYTES, kk * 16, Cfg::V_BOX), 1);
-    if (kMerge && next) issue_s(i + 1);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(o);
-    fence_regs(a);
-    fence_regs(s);
-    release_v(i);
-    if (!kMerge && next) {
-      mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
-      wgmma_fence();
-      issue_s(i + 1);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(s);
-    }
-    if (next) release_k(i + 1);
-    __syncwarp();
-  }
-
-  // ---------------- epilogue: O * (1/N) vd 2^-e_p -> bf16 ----------------
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    const int qi = q_base + hh * 8;
-    if (qi - m0 < mrows) {
-      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (row0 + qi) * p.o_row_stride + (long long)h * p.o_head_stride;
-#pragma unroll
-      for (int nb = 0; nb < D / 8; ++nb)
-        *reinterpret_cast<uint32_t*>(orow + nb * 8 + 2 * t4) =
-            pack_bf16x2(scalbnf(o[nb * 4 + hh * 2] * c_o, e_o), scalbnf(o[nb * 4 + hh * 2 + 1] * c_o, e_o));
-    }
-  }
+  attn_fwd_e4m3_body<D, D>(p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -294,8 +20,10 @@ static bool e4m3_view(const void* ptr, long long row_stride, long long head_stri
 }
 
 int e4m3_fwd_check(const hstu_attn_params& p) {
-  if (p.dqk != p.dv || (p.dqk != 32 && p.dqk != 64 && p.dqk != 128 && p.dqk != 256)) {
-    set_error("fp8 attention: dqk == dv in {32, 64, 128, 256} only (dqk=%d, dv=%d)", p.dqk, p.dv);
+  // dqk == dv, or dqk < dv (attn_wgmma_mixed_fwd_e4m3.cu), both in {32, 64, 128, 256}
+  auto dim_ok = [](int d) { return d == 32 || d == 64 || d == 128 || d == 256; };
+  if (p.dqk > p.dv || !dim_ok(p.dqk) || !dim_ok(p.dv)) {
+    set_error("fp8 attention: dqk == dv or dqk < dv, both in {32, 64, 128, 256}, only (dqk=%d, dv=%d)", p.dqk, p.dv);
     return HSTU_ERR_UNSUPPORTED;
   }
   if (p.delta_q_len != 0 || p.pos_w != nullptr || p.ts_w != nullptr) {
@@ -319,50 +47,20 @@ int e4m3_fwd_check(const hstu_attn_params& p) {
 }
 
 template <int D>
-static int launch_fwd_e4m3(const hstu_attn_params& p, const hstu_attn_descales& ds, const void* v16, cudaStream_t st) {
-  using Cfg = E4m3FwdCfg<D>;
-  E4m3FwdParams fp;
-  memset(&fp, 0, sizeof(fp));
-  if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, p.total_rows, p.heads, D, p.q_row_stride, p.q_head_stride, Cfg::QK_BOX_COLS, Cfg::BM, 1))
-    return e;
-  if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, D, p.k_row_stride, p.k_head_stride, Cfg::QK_BOX_COLS, Cfg::BN, 1))
-    return e;
-  if (int e = make_tmap_rows_heads(&fp.tmV, v16, p.total_rows, p.heads, D, (long long)p.heads * D, D, Cfg::V_BOX_COLS, Cfg::BN, 2))
-    return e;
-  fp.seq_offsets = p.seq_offsets;
-  fp.num_targets = p.num_targets;
-  fp.out = p.out;
-  fp.o_row_stride = p.o_row_stride;
-  fp.o_head_stride = p.o_head_stride;
-  fp.descale[0] = ds.q, fp.ds_batch[0] = ds.q_batch_stride, fp.ds_head[0] = ds.q_head_stride;
-  fp.descale[1] = ds.k, fp.ds_batch[1] = ds.k_batch_stride, fp.ds_head[1] = ds.k_head_stride;
-  fp.descale[2] = ds.v, fp.ds_batch[2] = ds.v_batch_stride, fp.ds_head[2] = ds.v_head_stride;
-  fp.offsets_i64 = p.offsets_are_i64;
-  fp.targets_i64 = p.num_targets_are_i64;
-  fp.max_seq_len = p.max_seq_len;
-  fp.win = p.max_attn_len;
-  fp.min_full = p.min_full_attn_seq_len;
-  fp.ctx = p.contextual_seq_len;
-  fp.alpha_half = 0.5f * p.alpha;
-  fp.alpha = p.alpha;
-  fp.inv_n = 1.0f / (float)p.max_seq_len;
-  auto kern = attn_fwd_e4m3_wgmma_kernel<D>;
-  HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  dim3 grid((p.max_seq_len + Cfg::BM - 1) / Cfg::BM, p.heads, p.batch);
-  kern<<<grid, kE4m3Threads, Cfg::SMEM_BYTES, st>>>(fp);
-  HSTU_CUDA_OK(cudaGetLastError());
-  return 0;
+static int launch_square(const hstu_attn_params& p, const hstu_attn_descales& ds, const void* v16, cudaStream_t st) {
+  return launch_fwd_e4m3<D, D>(p, ds, v16, st, attn_fwd_e4m3_wgmma_kernel<D>);
 }
 
 int attn_wgmma_fwd_e4m3(const hstu_attn_params& p, const hstu_attn_descales& ds, cudaStream_t st) {
   if (int e = e4m3_fwd_check(p)) return e;
   const void* v16 = nullptr;
   if (int e = e4m3_v_prepass(p, &v16, st)) return e;
+  if (p.dqk != p.dv) return attn_wgmma_fwd_e4m3_mixed(p, ds, v16, st);
   switch (p.dqk) {
-    case 32: return launch_fwd_e4m3<32>(p, ds, v16, st);
-    case 64: return launch_fwd_e4m3<64>(p, ds, v16, st);
-    case 128: return launch_fwd_e4m3<128>(p, ds, v16, st);
-    case 256: return launch_fwd_e4m3<256>(p, ds, v16, st);
+    case 32: return launch_square<32>(p, ds, v16, st);
+    case 64: return launch_square<64>(p, ds, v16, st);
+    case 128: return launch_square<128>(p, ds, v16, st);
+    case 256: return launch_square<256>(p, ds, v16, st);
   }
   set_error("fp8 attention: unsupported head dim %d", p.dqk);
   return HSTU_ERR_UNSUPPORTED;

@@ -42,6 +42,8 @@ int e4m3_v_prepass(const hstu_attn_params& p, const void** v16, cudaStream_t st)
 // alignment only, no device query), else HSTU_ERR_UNSUPPORTED with a message
 int e4m3_fwd_check(const hstu_attn_params& p);
 int attn_wgmma_fwd_e4m3(const hstu_attn_params& p, const hstu_attn_descales& ds, cudaStream_t st);
+// attn_wgmma_mixed_fwd_e4m3.cu: its dqk < dv kernels, on the fp16 copy v16 of v that attn_wgmma_fwd_e4m3 has written
+int attn_wgmma_fwd_e4m3_mixed(const hstu_attn_params& p, const hstu_attn_descales& ds, const void* v16, cudaStream_t st);
 bool is_sm90();
 
 // norm.cu

@@ -110,7 +110,8 @@ def cuda_hstu_attention_fwd_fp8(
     """Forward of attention on float8_e4m3fn q, k, v (`hstu_attn_fwd_fp8`): the bf16 result of the attention of
     q * q_descale[b, h], k * k_descale[b, h] and v * v_descale[b, h], every mask option of the bf16 path included.  Each
     descale is an fp32 [B, H] tensor (any strides) or None for 1.  There is no fp8 backward.  The wgmma kernels take
-    dqk == dv in {32, 64, 128, 256}, 16-byte aligned views with row / head strides that are multiples of 16 elements."""
+    dqk == dv, or dqk < dv, with both in {32, 64, 128, 256} (the output has dv columns), 16-byte aligned views with row /
+    head strides that are multiples of 16 elements."""
     if not all(t.dtype == _FP8 for t in (q, k, v)):
         raise RuntimeError(f"fp8 attention: q, k and v must all be torch.float8_e4m3fn (got {q.dtype}, {k.dtype}, {v.dtype}); "
                            "descales apply to fp8 inputs only")

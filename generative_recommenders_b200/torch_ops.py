@@ -10,8 +10,9 @@ Arguments this backend does not implement raise instead of being ignored: `attn_
 (`seq_offsets=None`).
 fp8: with q, k and v of dtype float8_e4m3fn, `hstu_mha_fwd` and `hstu_mha` run the fp8 forward (`hstu_attn_fwd_fp8`) and
 return bf16: the attention of q * q_descale[b, h], k * k_descale[b, h], v * v_descale[b, h], each descale an fp32 [B, H]
-tensor or None for 1, as in the reference's e4m3 forward.  There is no fp8 backward: `hstu_mha` raises when a gradient is
-requested through fp8 inputs.  Descales with bf16 / fp16 inputs raise.
+tensor or None for 1, as in the reference's e4m3 forward.  Head dims: dqk == dv, or dqk < dv (the DLRM-HSTU default
+attention_dim 128 / hidden_dim 256 included), both in {32, 64, 128, 256}.  There is no fp8 backward: `hstu_mha` raises when a
+gradient is requested through fp8 inputs.  Descales with bf16 / fp16 inputs raise.
 `deterministic=True` (or `torch.use_deterministic_algorithms(True)`) makes the backward bitwise reproducible: the wgmma
 backward then runs its atomic-free dK / dV and dQ kernels, and shapes it does not cover run the generic kernels, which have
 no atomics either.  Otherwise the wgmma backward at d = 64 / 128 accumulates dQ with fp32 atomic adds whose order varies

@@ -141,9 +141,10 @@ typedef struct hstu_attn_descales {
 } hstu_attn_descales;
 /* Forward of fp8 attention (the reference's e4m3 forward, flash_api.cpp hstu_mha_fwd with q/k/v_descale): p->dtype is
  * HSTU_E4M3 and out is bf16; out = attention(q * q_descale[b, h], k * k_descale[b, h], v * v_descale[b, h]) with every
- * mask option of hstu_attn_fwd.  wgmma kernels only (sm_90): dqk == dv in {32, 64, 128, 256}, no delta_q, no relative
- * bias; q / k / v bases 16-byte aligned with row and head strides that are multiples of 16 elements.  Other shapes
- * return HSTU_ERR_UNSUPPORTED.  Needs a workspace of hstu_attn_workspace_bytes(p, 0) bytes (an fp16 copy of v).
+ * mask option of hstu_attn_fwd.  wgmma kernels only (sm_90): dqk == dv, or dqk < dv, with both in {32, 64, 128, 256}
+ * (out has dv columns), no delta_q, no relative bias; q / k / v bases 16-byte aligned with row and head strides that are
+ * multiples of 16 elements.  Other shapes (dqk > dv among them) return HSTU_ERR_UNSUPPORTED.  Needs a workspace of
+ * hstu_attn_workspace_bytes(p, 0) bytes (an fp16 copy of v, L * H * dv * 2 rounded up to 256).
  * descales may be NULL (all scales 1). */
 int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* descales, void* cuda_stream);
 /* Which implementation a call would dispatch to: returns HSTU_IMPL_GENERIC or HSTU_IMPL_UMMA (<0 on error).  A

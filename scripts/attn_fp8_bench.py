@@ -1,12 +1,14 @@
 """Forward attention on fp8 (e4m3) inputs against bf16 and fp16 on the same values, in one process.
 
-    python scripts/attn_fp8_bench.py [--rounds 5] [--window 0.5] [--out FILE]
+    python scripts/attn_fp8_bench.py [--rounds 5] [--window 0.5] [--mixed-dims] [--out FILE]
 
 Inputs: `bench.py`'s length recipe (`synth_lengths`: lengths U[0.9, 1) Lmax with 1-20 targets, seed 1001); q, k ~ N(0, 1)
 and v ~ N(0, 1), alpha = 1/sqrt(d) (rms(alpha S) = 1).  q, k, v are quantised per (sequence, head) with descale = amax / 448;
 the bf16 and fp16 arms run on the dequantised values (x8 * descale) rounded to their dtype.  Shapes (d, Lmax, sequences,
 heads): the headline attention d = 32 at 8192 / 16 / 8, and d = 64 at 2048 / 128, d = 128 at 4096 / 32, d = 256 at
-1024 / 128, all with 4 heads.
+1024 / 128, all with 4 heads.  `--mixed-dims` runs the dqk < dv cells instead, with the batches of attn_mixed_dims_bench.py:
+(128, 256) at Lmax 512 / 2048 / 8192 with 512 / 128 / 16 sequences, and (32, 64), (32, 128), (32, 256), (64, 128),
+(64, 256) at Lmax 2048 with 128 sequences, all with 4 heads; q, k have dqk columns, v has dv, and alpha = 1/sqrt(dqk).
 
 Each arm is warmed up.  Then, in every round, the three arms run one after another with CUDA events, each over enough
 back-to-back calls to fill `--window` seconds; medians over rounds are reported (wall-clock ms per call; the fp8 arm includes
@@ -34,7 +36,9 @@ import torch
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 
-SHAPES = [(32, 8192, 16, 8), (64, 2048, 128, 4), (128, 4096, 32, 4), (256, 1024, 128, 4)]
+SHAPES = [(32, 32, 8192, 16, 8), (64, 64, 2048, 128, 4), (128, 128, 4096, 32, 4), (256, 256, 1024, 128, 4)]  # (dqk, dv, ...)
+MIXED_SHAPES = [(128, 256, 512, 512, 4), (128, 256, 2048, 128, 4), (128, 256, 8192, 16, 4)] + [
+    (dqk, dv, 2048, 128, 4) for dqk, dv in [(32, 64), (32, 128), (32, 256), (64, 128), (64, 256)]]
 FP8 = torch.float8_e4m3fn
 
 
@@ -116,6 +120,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--window", type=float, default=0.5, help="seconds of back-to-back calls per timed window")
     ap.add_argument("--profile-rounds", type=int, default=2, help="alternated rounds of profiled sustained windows")
+    ap.add_argument("--mixed-dims", action="store_true", help="the dqk < dv cells (MIXED_SHAPES) instead of SHAPES")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     from bench import ensure_built, synth_lengths
@@ -137,18 +142,18 @@ def main():
         return e0.elapsed_time(e1) / n
 
     res = {"rounds": args.rounds, "window_s": args.window, "shapes": []}
-    for d, lmax, batch, heads in SHAPES:
+    for dqk, dv, lmax, batch, heads in (MIXED_SHAPES if args.mixed_dims else SHAPES):
         lengths, nt, off = synth_lengths(batch, lmax, dev, 1001)
         L = int(off[-1])
         g = torch.Generator(device=dev).manual_seed(3003)
-        q8, k8, v8 = (quantize(torch.randn(L, heads, d, device=dev, generator=g), off) for _ in range(3))
+        q8, k8, v8 = (quantize(torch.randn(L, heads, w, device=dev, generator=g), off) for w in (dqk, dqk, dv))
         ds = (q8[1], k8[1], v8[1])
         q8, k8, v8 = q8[0], k8[0], v8[0]
         o = off.tolist()
         rows = torch.repeat_interleave(torch.arange(batch, device=dev), torch.tensor([o[i + 1] - o[i] for i in range(batch)], device=dev))
         deq = [x.double() * dd.double()[rows][:, :, None] for x, dd in zip((q8, k8, v8), ds)]
         arms = {"fp8": (q8, k8, v8), "bf16": tuple(x.to(torch.bfloat16) for x in deq), "fp16": tuple(x.to(torch.float16) for x in deq)}
-        alpha = 1.0 / math.sqrt(d)
+        alpha = 1.0 / math.sqrt(dqk)
         outs = {}
 
         def call(name):
@@ -205,24 +210,26 @@ def main():
             kcycles[name] = statistics.median(r[1] * r[2] for r in rows_) if None not in (r[2] for r in rows_) else None
             kernels[name] = {k: statistics.median(r[3].get(k, 0.0) for r in rows_) for k in rows_[0][3]}
         prepass = sum(t for k, t in kernels["fp8"].items() if "convert_kernel" in k)
-        attn = sum(t for k, t in kernels["fp8"].items() if "e4m3_wgmma_kernel" in k)
+        attn = sum(t for k, t in kernels["fp8"].items() if "e4m3_wgmma_kernel" in k or "e4m3_mixed_wgmma_kernel" in k)
         row = {
-            "d": d, "lmax": lmax, "sequences": batch, "heads": heads, "rows": L, "calls_per_window": iters,
+            **({"d": dqk} if dqk == dv else {"dqk": dqk, "dv": dv}), "lmax": lmax, "sequences": batch, "heads": heads, "rows": L, "calls_per_window": iters,
             "ms_median": med, "ms_all": times, "fp8_over_bf16": med["fp8"] / med["bf16"], "fp8_over_fp16": med["fp8"] / med["fp16"],
             "sm_clock_mhz_median": clock_med, "power_w_median": power_med,
             "kernel_ms_per_call": kernel_ms, "kernel_fp8_over_bf16": kernel_ms["fp8"] / kernel_ms["bf16"],
             "kernel_fp8_over_fp16": kernel_ms["fp8"] / kernel_ms["fp16"], "device_idle_ms_per_call": idle_ms,
             "kernel_kilocycles_per_call": kcycles,
-            "profile_fp8_ms_per_call": {"prepass_v_to_fp16": prepass, "attention_kernel": attn},
+            "profile_fp8_ms_per_call": {"prepass_v_to_fp16": prepass, "attention_kernel": attn,
+                                        **({} if dqk == dv else {"prepass_share": prepass / (prepass + attn)})},
             "profile_kernels_ms_per_call": kernels,
             "rel_l2_vs_fp64_sampled": {name: max(e) for name, e in errs.items()},
             "finite": all(bool(torch.isfinite(x).all()) for x in outs.values()),
         }
         res["shapes"].append(row)
-        print(json.dumps({k: row[k] for k in ("d", "lmax", "ms_median", "fp8_over_bf16", "fp8_over_fp16", "sm_clock_mhz_median",
+        print(json.dumps({k: row[k] for k in ("d", "dqk", "dv", "lmax", "ms_median", "fp8_over_bf16", "fp8_over_fp16", "sm_clock_mhz_median",
                                                "power_w_median", "kernel_ms_per_call", "kernel_fp8_over_bf16",
                                                "kernel_fp8_over_fp16", "device_idle_ms_per_call", "kernel_kilocycles_per_call",
-                                               "profile_fp8_ms_per_call", "rel_l2_vs_fp64_sampled")}), file=sys.stderr, flush=True)
+                                               "profile_fp8_ms_per_call", "rel_l2_vs_fp64_sampled") if k in row}), file=sys.stderr,
+              flush=True)
         del arms, outs, deq
         torch.cuda.empty_cache()
     res["card"] = card()  # read right after the timing, so the SM clock is the loaded one
