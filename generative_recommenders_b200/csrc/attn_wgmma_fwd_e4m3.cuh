@@ -7,9 +7,9 @@
 //   out = attention(q * qd[b, h], k * kd[b, h], v * vd[b, h])
 //
 // The structure is the bf16 / fp16 forward's (attn_wgmma_fwd.cuh): one CTA per (128-row query tile, head, sequence), heavy
-// tiles first; two warpgroups of 64 query rows; 64-key tiles through a ring of STAGES K and V buffers, refilled by the warp
-// whose release is the last of the eight (release_is_last, the same protocol); tile-uniform mask cases; where kMerge, O +=
-// P_i V_i and S_{i+1} = Q K_{i+1}^T form one MMA batch with one wait.  What differs:
+// tiles first; two warpgroups of 64 query rows; the prologue, the K / V ring protocol of 64-key tiles and the tile-uniform
+// mask cases of attn_wgmma_qtile.cuh; where kMerge, O += P_i V_i and S_{i+1} = Q K_{i+1}^T form one MMA batch with one
+// wait.  What differs:
 //   S = Q K^T  on fp8 tensor cores (wgmma m64n64k32 e4m3, both operands K-major).  Q and K are TMA-staged as bytes; a row
 //              of dqk e4m3 values has the layout of a 16-bit row of dqk / 2, so the K-major descriptors apply with 32-byte k
 //              steps.  Swizzle: 32 B at dqk = 32, 64 B at dqk = 64, 128-byte boxes at dqk >= 128.
@@ -25,6 +25,7 @@
 #include <string.h>
 
 #include "attn_fp16_operands.cuh"
+#include "attn_wgmma_qtile.cuh"
 #include "common.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
@@ -34,16 +35,11 @@ using namespace wg;
 
 struct alignas(64) E4m3FwdParams {
   CUtensorMap tmQ, tmK, tmV;  // Q, K: the e4m3 inputs (bytes); V: the fp16 copy of v
-  const void* seq_offsets;
-  const void* num_targets;
+  SeqArgs seq;
   void* out;  // bf16
   long long o_row_stride, o_head_stride;
   const float* descale[3];  // q, k, v: [B, H] fp32, or null (= 1)
   long long ds_batch[3], ds_head[3];
-  int offsets_i64, targets_i64;
-  int max_seq_len;
-  int win, min_full, ctx;
-  float alpha_half;  // alpha / 2
   float alpha;
   float inv_n;       // 1 / max_seq_len
 };
@@ -52,10 +48,10 @@ template <int DQK, int DV = DQK>
 struct E4m3FwdCfg {
   static constexpr int BM = 128;  // query rows per CTA (two warpgroups of 64)
   static constexpr int BN = 64;   // key rows per tile
-  static constexpr int SWK = DQK >= 128 ? 128 : DQK;        // swizzle (bytes) of the e4m3 Q / K boxes: one byte per element
-  static constexpr int SWV = 2 * DV >= 128 ? 128 : 2 * DV;  // of the fp16 V boxes
-  static constexpr int QK_BOX_COLS = SWK, V_BOX_COLS = SWV / 2;
-  static constexpr int NBOX_QK = DQK / QK_BOX_COLS, NBOX_V = DV / V_BOX_COLS;
+  static constexpr int SWK = swizzle_bytes(DQK, 1);  // swizzle (bytes) of the e4m3 Q / K boxes: one byte per element
+  static constexpr int SWV = swizzle_bytes(DV);      // of the fp16 V boxes
+  static constexpr int BOX_COLS = SWK, BOX_COLS_V = SWV / 2;
+  static constexpr int NBOX = DQK / BOX_COLS, NBOX_V = DV / BOX_COLS_V;
   static constexpr int Q_BOX = BM * SWK, K_BOX = BN * SWK, V_BOX = BN * SWV;
   static constexpr int Q_BYTES = BM * DQK, K_BYTES = BN * DQK, V_BYTES = BN * DV * 2;
   static constexpr int STAGES = 3;  // 128 dqk + 3 (64 dqk + 128 dv) bytes: 136 KB at (128, 256), 177 KB at d = 256
@@ -68,18 +64,11 @@ struct E4m3FwdCfg {
   static_assert(OFF_K % 1024 == 0 && OFF_V % 1024 == 0 && K_BYTES % 256 == 0 && V_BYTES % 1024 == 0, "swizzle atom alignment");
   static_assert(DQK <= DV, "dqk > dv has no instantiation");
 };
-constexpr int kE4m3Threads = 256;
 // dv <= 64: two CTAs per SM (<= 128 registers per thread), and S_{i+1} merged into the P_i V_i batch.  The O accumulator is
 // dv / 2 registers per thread, so every pair with dv >= 128 runs one CTA per SM and waits for each batch separately
 // (ptxas -v of each choice: DESIGN.md 3.5)
 template <int DV> constexpr int kE4m3MinBlocks = (DV <= 64) ? 2 : 1;
 template <int DV> constexpr bool kE4m3Merge = DV <= 64;
-
-struct E4m3Bars {
-  uint64_t q_full;
-  uint64_t k_full[3], v_full[3];
-  uint32_t k_free[3], v_free[3];  // release counters of the K / V stages (release_is_last: one arrival per warp and use)
-};
 
 __device__ __forceinline__ float load_descale(const float* d, long long bs, long long hs, int b, int h) {
   return d ? d[(long long)b * bs + (long long)h * hs] : 1.f;
@@ -93,72 +82,44 @@ __device__ __forceinline__ void attn_fwd_e4m3_body(const E4m3FwdParams& p) {
   constexpr bool kMerge = kE4m3Merge<DV>;  // as in the bf16 forward: S_{i+1} and P_i V_i in one batch where the registers allow
   const int b = blockIdx.z, h = blockIdx.y;
   const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
-  const long long row0 = load_index(p.seq_offsets, p.offsets_i64, b);
-  int len = (int)(load_index(p.seq_offsets, p.offsets_i64, b + 1) - row0);
-  if (len > p.max_seq_len) {  // rows past max_seq_len are ignored on the way in and zero on the way out
-    if (blockIdx.x == 0) zero_rows(p.out, 2, p.o_row_stride, (long long)h * p.o_head_stride, DV, row0 + p.max_seq_len, row0 + len);
-    len = p.max_seq_len;
-  }
-  if (m0 >= len) return;
-  const int n_tgt = p.num_targets ? (int)load_index(p.num_targets, p.targets_i64, b) : -1;
-  const SeqMask msk = make_seq_mask(len, n_tgt, p.win, p.min_full, p.ctx);
-  const int mrows = min(Cfg::BM, len - m0);
-  int lo, hi;
-  kv_range_for_q_rows(msk, m0, m0 + mrows, &lo, &hi);
-  const int t0 = lo / BN;
-  const int T = (hi + BN - 1) / BN - t0;  // >= 1 (the diagonal tile)
+  QTileSeq qs;
+  if (!qtile_prologue<Cfg::BM, BN>(p.seq, b, h, m0, p.out, p.o_row_stride, p.o_head_stride, DV, &qs)) return;
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  E4m3Bars* bars = reinterpret_cast<E4m3Bars*>(smem + Cfg::OFF_BAR);
+  uint8_t* smem = dyn_smem_1k();
+  KvRing<Cfg> ring{smem, &p.tmK, &p.tmV, h, qs.row0, qs.t0, qs.T};
+  ring.init();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(&bars->q_full, 1);
-    for (int i = 0; i < NST; ++i) {
-      mbar_init(&bars->k_full[i], 1);
-      mbar_init(&bars->v_full[i], 1);
-      bars->k_free[i] = bars->v_free[i] = 0u;
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  const int key_row0 = (int)(row0 + (long long)t0 * BN);
-  auto load_k = [&](int i) {
+  // The protocol of KvRing (barriers, waits, release_is_last), but this loop issues the fill and the refills itself: the
+  // stage of each load is recomputed from its tile index, and the key row is 32-bit.  KvRing::fill / release take the
+  // caller's stage, which makes ptxas keep this loop's ring state in vector rather than uniform registers (up to +23
+  // registers and +3 instructions per tile), and KvRing::load's 64-bit row costs a uniform -> vector -> uniform round trip
+  // per TMA box of every refill (DESIGN.md 3.5).
+  const int key_row0 = (int)(qs.row0 + (long long)qs.t0 * BN);
+  auto load = [&](auto val_c, int i) {
+    constexpr bool kIsV = decltype(val_c)::value;
     const int st = i % NST;
-    mbar_arrive_expect_tx(&bars->k_full[st], Cfg::K_BYTES);
+    uint64_t* full = kIsV ? ring.bars->v_full : ring.bars->k_full;
+    mbar_arrive_expect_tx(&full[st], kIsV ? Cfg::V_BYTES : Cfg::K_BYTES);
 #pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX_QK; ++bx)
-      tma_load_3d(smem + Cfg::OFF_K + st * Cfg::K_BYTES + bx * Cfg::K_BOX, &p.tmK, &bars->k_full[st], bx * Cfg::QK_BOX_COLS, h,
-                  key_row0 + i * BN);
+    for (int bx = 0; bx < (kIsV ? Cfg::NBOX_V : Cfg::NBOX); ++bx)
+      tma_load_3d(smem + (kIsV ? Cfg::OFF_V + st * Cfg::V_BYTES + bx * Cfg::V_BOX : Cfg::OFF_K + st * Cfg::K_BYTES + bx * Cfg::K_BOX),
+                  kIsV ? &p.tmV : &p.tmK, &full[st], bx * (kIsV ? Cfg::BOX_COLS_V : Cfg::BOX_COLS), h, key_row0 + i * BN);
   };
-  auto load_v = [&](int i) {
-    const int st = i % NST;
-    mbar_arrive_expect_tx(&bars->v_full[st], Cfg::V_BYTES);
-#pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX_V; ++bx)
-      tma_load_3d(smem + Cfg::OFF_V + st * Cfg::V_BYTES + bx * Cfg::V_BOX, &p.tmV, &bars->v_full[st], bx * Cfg::V_BOX_COLS, h,
-                  key_row0 + i * BN);
-  };
-  // the ring protocol of the bf16 forward: each warp releases the K (V) stage of tile i once its MMAs that read it have
-  // completed, and the warp whose release is the last of the eight loads tile i + STAGES into it
-  auto release_k = [&](int i) {
-    if (lane == 0 && i + NST < T && release_is_last<kE4m3Threads / 32>(&bars->k_free[i % NST])) load_k(i + NST);
-  };
-  auto release_v = [&](int i) {
-    if (lane == 0 && i + NST < T && release_is_last<kE4m3Threads / 32>(&bars->v_free[i % NST])) load_v(i + NST);
+  auto release = [&](auto val_c, int i) {
+    uint32_t* ctr = decltype(val_c)::value ? ring.bars->v_free : ring.bars->k_free;
+    if (lane == 0 && i + NST < qs.T && release_is_last<kAttnThreads / 32>(&ctr[i % NST])) load(val_c, i + NST);
   };
   if (tid == 0) {
     prefetch_tensormap(&p.tmQ);
     prefetch_tensormap(&p.tmK);
     prefetch_tensormap(&p.tmV);
-    mbar_arrive_expect_tx(&bars->q_full, Cfg::Q_BYTES);
+    mbar_arrive_expect_tx(&ring.bars->q_full, Cfg::Q_BYTES);
 #pragma unroll
-    for (int bx = 0; bx < Cfg::NBOX_QK; ++bx)
-      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &bars->q_full, bx * Cfg::QK_BOX_COLS, h, (int)(row0 + m0));
-    for (int i = 0; i < min(T, NST); ++i) {
-      load_k(i);
-      load_v(i);
+    for (int bx = 0; bx < Cfg::NBOX; ++bx)
+      tma_load_3d(smem + Cfg::OFF_Q + bx * Cfg::Q_BOX, &p.tmQ, &ring.bars->q_full, bx * Cfg::BOX_COLS, h, (int)(qs.row0 + m0));
+    for (int i = 0; i < min(qs.T, NST); ++i) {
+      load(kKey, i);
+      load(kVal, i);
     }
   }
   __syncwarp();
@@ -167,8 +128,8 @@ __device__ __forceinline__ void attn_fwd_e4m3_body(const E4m3FwdParams& p) {
   const int q_base = m0 + wgi * 64 + w * 16 + g;  // query position of accumulator rows g (+ 8)
   const uint32_t sq = smem_u32(smem + Cfg::OFF_Q) + wgi * 64 * SWK;
   const uint32_t sk = smem_u32(smem + Cfg::OFF_K), sv = smem_u32(smem + Cfg::OFF_V);
-  const bool fast = msk.fast != 0;
-  const int full_lim = fast ? min(m0, msk.has_tgt ? msk.max_id : 0x7fffffff) : -1;  // keys < full_lim: valid for every row
+  const bool fast = qs.msk.fast != 0;
+  const int full_lim = full_valid_limit(qs.msk, m0);
   // scales of this (sequence, head): S holds S / (qd kd), P is formed as 2^e_p P, O holds 2^e_p O / vd.
   const float qd = load_descale(p.descale[0], p.ds_batch[0], p.ds_head[0], b, h);
   const float kd = load_descale(p.descale[1], p.ds_batch[1], p.ds_head[1], b, h);
@@ -181,7 +142,7 @@ __device__ __forceinline__ void attn_fwd_e4m3_body(const E4m3FwdParams& p) {
   // The bound of e_p is on |alpha qd kd S|, and S sums dqk products: it takes dqk, whatever dv is.
   const int e_p = e4m3_p_exp(p.alpha, qd, kd, DQK);
   int ea, eq, ek, ev;
-  const float m_s = frexpf(p.alpha_half, &ea) * frexpf(qd, &eq) * frexpf(kd, &ek);
+  const float m_s = frexpf(p.seq.alpha_half, &ea) * frexpf(qd, &eq) * frexpf(kd, &ek);
   const float c_s = scalbnf(m_s, ea + eq + ek), c_sp = scalbnf(m_s, ea + eq + ek + e_p);
   const float c_o = p.inv_n * frexpf(vd, &ev);
   const int e_o = ev - e_p;
@@ -204,61 +165,34 @@ __device__ __forceinline__ void attn_fwd_e4m3_body(const E4m3FwdParams& p) {
       wgmma_ss_64_e4m3(s, desc_kmajor<SWK>(sq + bx * Cfg::Q_BOX, off), desc_kmajor<SWK>(kst + bx * Cfg::K_BOX, off), ks > 0);
     }
   };
-  mbar_wait(&bars->q_full, 0);
-  mbar_wait(&bars->k_full[0], 0);
+  mbar_wait(&ring.bars->q_full, 0);
+  ring.wait(kKey, 0, 0);
   wgmma_fence();
   issue_s(0);
   wgmma_commit();
   wgmma_wait<0>();
   fence_regs(s);
-  release_k(0);
+  release(kKey, 0);
   __syncwarp();
-  for (int i = 0; i < T; ++i) {
+  for (int i = 0; i < qs.T; ++i) {
     const int st = i % NST;
-    const bool next = i + 1 < T;
-    const int n0 = (t0 + i) * BN;
+    const bool next = i + 1 < qs.T;
+    const int n0 = (qs.t0 + i) * BN;
     // P' = 2^e_p silu(alpha S) * mask; the mask case is chosen once per tile, so each score loop is one basic block
     auto silu = [&](int n) {
       const float x = s[n] * c_s, xp = s[n] * c_sp;
       return __fmaf_rn(xp, tanh_approx(x), xp);  // silu(2x) = x (1 + tanh x)
     };
-    if (n0 + BN <= full_lim) {  // tile-uniform: every pair valid
-#pragma unroll
-      for (int n = 0; n < BN / 2; ++n) s[n] = silu(n);
-    } else if (fast) {
-      int lim[2];
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) lim[hh] = msk.has_tgt ? min(q_base + hh * 8, msk.max_id) : q_base + hh * 8;
-#pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float pv = silu(nb * 4 + e);
-          s[nb * 4 + e] = (kj < len && (kj < lim[e >> 1] || kj == qi)) ? pv : 0.f;
-        }
-    } else {
-#pragma unroll
-      for (int nb = 0; nb < BN / 8; ++nb)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
-          const float pv = silu(nb * 4 + e);
-          s[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? pv : 0.f;
-        }
-    }
+    mask_scores<BN>(qs.msk, fast, full_lim, qs.len, q_base, n0, t4, s, silu);
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk)
 #pragma unroll
       for (int r = 0; r < 4; ++r) a[kk][r] = pack_f16x2_sat(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
-    mbar_wait(&bars->v_full[st], (i / NST) & 1);
+    ring.wait(kVal, st, (i / NST) & 1);
     // the last tile may cross the sequence end: its V rows >= len belong to the next sequence (P is 0 there, V may be NaN)
-    if (n0 + BN > len) {  // CTA-uniform; the last tile, so its stage is not refilled
-      zero_tile_rows<BN, SWV, Cfg::NBOX_V, kE4m3Threads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, len - n0);
-      fence_proxy_async_smem();
-      named_bar_sync(kBarZeroRows, kE4m3Threads);
-    }
-    if (kMerge && next) mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+    if (n0 + BN > qs.len)  // CTA-uniform; the last tile, so its stage is not refilled
+      zero_tile_rows_sync<BN, SWV, Cfg::NBOX_V, kAttnThreads>(smem + Cfg::OFF_V + st * Cfg::V_BYTES, qs.len - n0);
+    if (kMerge && next) ring.wait(kKey, (i + 1) % NST, ((i + 1) / NST) & 1);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk)
@@ -269,16 +203,16 @@ __device__ __forceinline__ void attn_fwd_e4m3_body(const E4m3FwdParams& p) {
     fence_regs(o);
     fence_regs(a);
     fence_regs(s);
-    release_v(i);
+    release(kVal, i);
     if (!kMerge && next) {
-      mbar_wait(&bars->k_full[(i + 1) % NST], ((i + 1) / NST) & 1);
+      ring.wait(kKey, (i + 1) % NST, ((i + 1) / NST) & 1);
       wgmma_fence();
       issue_s(i + 1);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(s);
     }
-    if (next) release_k(i + 1);
+    if (next) release(kKey, i + 1);
     __syncwarp();
   }
 
@@ -286,8 +220,8 @@ __device__ __forceinline__ void attn_fwd_e4m3_body(const E4m3FwdParams& p) {
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int qi = q_base + hh * 8;
-    if (qi - m0 < mrows) {
-      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (row0 + qi) * p.o_row_stride + (long long)h * p.o_head_stride;
+    if (qi - m0 < qs.mrows) {
+      uint16_t* orow = reinterpret_cast<uint16_t*>(p.out) + (qs.row0 + qi) * p.o_row_stride + (long long)h * p.o_head_stride;
 #pragma unroll
       for (int nb = 0; nb < DV / 8; ++nb)
         *reinterpret_cast<uint32_t*>(orow + nb * 8 + 2 * t4) =
@@ -306,32 +240,24 @@ int launch_fwd_e4m3(const hstu_attn_params& p, const hstu_attn_descales& ds, con
   using Cfg = E4m3FwdCfg<DQK, DV>;
   E4m3FwdParams fp;
   memset(&fp, 0, sizeof(fp));
-  if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, p.total_rows, p.heads, DQK, p.q_row_stride, p.q_head_stride, Cfg::QK_BOX_COLS, Cfg::BM, 1))
+  if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, p.total_rows, p.heads, DQK, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BM, 1))
     return e;
-  if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, DQK, p.k_row_stride, p.k_head_stride, Cfg::QK_BOX_COLS, Cfg::BN, 1))
+  if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, DQK, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BN, 1))
     return e;
-  if (int e = make_tmap_rows_heads(&fp.tmV, v16, p.total_rows, p.heads, DV, (long long)p.heads * DV, DV, Cfg::V_BOX_COLS, Cfg::BN, 2))
+  if (int e = make_tmap_rows_heads(&fp.tmV, v16, p.total_rows, p.heads, DV, (long long)p.heads * DV, DV, Cfg::BOX_COLS_V, Cfg::BN, 2))
     return e;
-  fp.seq_offsets = p.seq_offsets;
-  fp.num_targets = p.num_targets;
+  fp.seq = seq_args(p);
   fp.out = p.out;
   fp.o_row_stride = p.o_row_stride;
   fp.o_head_stride = p.o_head_stride;
   fp.descale[0] = ds.q, fp.ds_batch[0] = ds.q_batch_stride, fp.ds_head[0] = ds.q_head_stride;
   fp.descale[1] = ds.k, fp.ds_batch[1] = ds.k_batch_stride, fp.ds_head[1] = ds.k_head_stride;
   fp.descale[2] = ds.v, fp.ds_batch[2] = ds.v_batch_stride, fp.ds_head[2] = ds.v_head_stride;
-  fp.offsets_i64 = p.offsets_are_i64;
-  fp.targets_i64 = p.num_targets_are_i64;
-  fp.max_seq_len = p.max_seq_len;
-  fp.win = p.max_attn_len;
-  fp.min_full = p.min_full_attn_seq_len;
-  fp.ctx = p.contextual_seq_len;
-  fp.alpha_half = 0.5f * p.alpha;
   fp.alpha = p.alpha;
   fp.inv_n = 1.0f / (float)p.max_seq_len;
   HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   dim3 grid((p.max_seq_len + Cfg::BM - 1) / Cfg::BM, p.heads, p.batch);
-  kern<<<grid, kE4m3Threads, Cfg::SMEM_BYTES, st>>>(fp);
+  kern<<<grid, kAttnThreads, Cfg::SMEM_BYTES, st>>>(fp);
   HSTU_CUDA_OK(cudaGetLastError());
   return 0;
 }

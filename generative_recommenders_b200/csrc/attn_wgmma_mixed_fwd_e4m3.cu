@@ -8,7 +8,7 @@
 namespace hstu {
 
 template <int DQK, int DV>
-__global__ void __launch_bounds__(kE4m3Threads, kE4m3MinBlocks<DV>) attn_fwd_e4m3_mixed_wgmma_kernel(const __grid_constant__ E4m3FwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, kE4m3MinBlocks<DV>) attn_fwd_e4m3_mixed_wgmma_kernel(const __grid_constant__ E4m3FwdParams p) {
   attn_fwd_e4m3_body<DQK, DV>(p);
 }
 

@@ -1,9 +1,9 @@
-// What the query-stationary 16-bit wgmma attention kernels share around their MMAs: the forward (attn_wgmma_fwd.cuh) and the
-// split backward's dQ kernel (attn_wgmma_bwd.cuh).  Each keeps a 128-row query tile
-// resident (two warpgroups of 64 rows) and streams the key tiles its rows attend through a ring of K and V stages.  Here, once:
-// the sequence arguments and the prologue that turns them into the CTA's rows and key tiles, the K / V ring, and the
-// choice of the mask case per tile.  The tile loops (MMA order, waits,
-// what is released when) differ for reasons given at each kernel and stay there.
+// What the query-stationary wgmma attention kernels share around their MMAs: the bf16 / fp16 forward (attn_wgmma_fwd.cuh),
+// the split backward's dQ kernel (attn_wgmma_bwd.cuh) and the fp8 forward (attn_wgmma_fwd_e4m3.cuh).  Each keeps a 128-row
+// query tile resident (two warpgroups of 64 rows) and streams the key tiles its rows attend through a ring of K and V
+// stages.  Here, once: the sequence arguments and the prologue that turns them into the CTA's rows and key tiles, the K / V
+// ring, and the choice of the mask case per tile.  The tile loops (MMA order, waits, what is released when) differ for
+// reasons given at each kernel and stay there.
 #pragma once
 #include <type_traits>
 
@@ -16,7 +16,7 @@ using namespace wg;
 
 constexpr int kAttnThreads = 256;  // every wgmma attention kernel: two warpgroups
 
-// The jagged layout, head count and mask of a call, as the 16-bit wgmma attention kernels take them.  (The order keeps the
+// The jagged layout, head count and mask of a call, as the wgmma attention kernels take them.  (The order keeps the
 // pairs of 32-bit fields that the backward kernels read with one 64-bit constant load.)
 struct SeqArgs {
   const void* seq_offsets;

@@ -285,17 +285,31 @@ def report():
     sr = _sass_report()
     if sr.tools() is None:
         pytest.skip("nvcc / cuobjdump not installed")
-    return sr.report("attn_fwd_e4m3_wgmma_kernel")
+    return sr.report("attn_fwd_e4m3")
+
+
+def _check_schedule(report, name, dv):
+    """No spills, no wgmma serialisation, and no more registers or per-tile instructions than the kernels compiled to when
+    each carried its own copy of the K / V ring (CUDA 12.9, the flags of build.py): <= 128 registers at dv <= 64 (two CTAs
+    per SM), 210 instructions per tile with the merged MMA batch (dv <= 64) and 203 without."""
+    found = [r for n, r in report.items() if name in n]
+    assert len(found) == 1, (name, sorted(report))
+    r = found[0]
+    assert r["spill_stores"] == 0 and r["spill_loads"] == 0, r
+    assert not set(r["notes"]) & {"C7510", "C7512", "C7515"}, r
+    if dv <= 64:
+        assert r["registers"] <= 128, r
+    assert r["iter_instrs"] is not None and r["iter_instrs"] <= (210 if dv <= 64 else 203), r
+    return r
 
 
 @pytest.mark.parametrize("d", [32, 64, 128, 256])
 def test_e4m3_kernel_schedule(report, d):
-    found = [r for name, r in report.items() if f"attn_fwd_e4m3_wgmma_kernel<(int){d}>" in name]
-    assert len(found) == 1, (d, sorted(report))
-    r = found[0]
-    assert r["spill_stores"] == 0 and r["spill_loads"] == 0, r
-    assert not set(r["notes"]) & {"C7510", "C7512", "C7515"}, r
-    if d <= 64:  # two CTAs per SM
-        assert r["registers"] <= 128, r
+    r = _check_schedule(report, f"attn_fwd_e4m3_wgmma_kernel<(int){d}>", d)
     if d == 32:
         assert r["tanh_per_block"] >= 8, r
+
+
+@pytest.mark.parametrize("dqk,dv", [(32, 64), (32, 128), (32, 256), (64, 128), (64, 256), (128, 256)])
+def test_e4m3_mixed_kernel_schedule(report, dqk, dv):
+    _check_schedule(report, f"attn_fwd_e4m3_mixed_wgmma_kernel<(int){dqk}, (int){dv}>", dv)

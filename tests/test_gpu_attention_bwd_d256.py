@@ -183,6 +183,8 @@ def test_d256_stu_layer_vs_oracle():
     out = {}
 
     def run():
+        stack.zero_grad(set_to_none=True)
+        xd.grad = None
         y = stack(x=xd, x_lengths=torch.tensor(lengths, device=DEV), x_offsets=off.to(DEV), max_seq_len=N,
                   num_targets=torch.tensor(nts, device=DEV))
         y.backward(dout.to(DEV))
