@@ -73,6 +73,10 @@ _PROTOS = {
     "hstu_attn_bwd": (C.c_int, [C.POINTER(AttnParams), _vp]),
     "hstu_attn_fwd_fp8": (C.c_int, [C.POINTER(AttnParams), C.POINTER(Descales), _vp]),
     "hstu_attn_select_impl": (C.c_int, [C.POINTER(AttnParams), C.c_int]),
+    "hstu_attn_fp16_operands_bytes": (C.c_size_t, [C.POINTER(AttnParams)]),
+    "hstu_attn_fwd_keep_fp16_operands": (C.c_int, [C.POINTER(AttnParams), _vp, C.c_size_t, _vp]),
+    "hstu_attn_bwd_fp16_operands_workspace_bytes": (C.c_size_t, [C.POINTER(AttnParams)]),
+    "hstu_attn_bwd_on_fp16_operands": (C.c_int, [C.POINTER(AttnParams), _vp, C.c_size_t, _vp]),
     "hstu_mask_valid": (C.c_int, [_i32] * 7),
     "hstu_kv_range_for_q_rows": (C.c_int, [_i32] * 7 + [C.POINTER(_i32)] * 2),
     "hstu_q_range_for_kv_rows": (C.c_int, [_i32] * 7 + [C.POINTER(_i32)] * 3),

@@ -92,6 +92,11 @@ static int select_impl(const hstu_attn_params* p, bool bwd) {
   return can ? HSTU_IMPL_UMMA : HSTU_IMPL_GENERIC;
 }
 
+// The calls that run on scaled fp16 operands (attn_fp16_operands.cu): bf16 at dqk == dv == 32 on the wgmma kernels
+static bool runs_on_fp16_operands(const hstu_attn_params* p, bool bwd) {
+  return p->dtype == HSTU_BF16 && p->dqk == 32 && p->dv == 32 && p->delta_q_len == 0 && select_impl(p, bwd) == HSTU_IMPL_UMMA;
+}
+
 // Nullable descales: no negative strides, fp32-aligned pointers.
 static int validate_descales(const hstu_attn_descales* d) {
   if (d == nullptr) return 0;
@@ -191,6 +196,59 @@ int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* desca
   hstu_attn_descales none;
   memset(&none, 0, sizeof(none));
   return attn_wgmma_fwd_e4m3(*p, descales ? *descales : none, (cudaStream_t)stream);
+}
+
+size_t hstu_attn_fp16_operands_bytes(const hstu_attn_params* p) {
+  if (p == nullptr || validate_attn(p, false) != 0) return 0;
+  if (p->batch == 0 || p->total_rows == 0 || !runs_on_fp16_operands(p, false)) return 0;
+  return fp16_operands_workspace_bytes(*p, false);
+}
+
+int hstu_attn_fwd_keep_fp16_operands(const hstu_attn_params* p, void* operands, size_t operands_bytes, void* stream) {
+  if (int e = validate_attn(p, false)) return e;
+  if (p->batch == 0 || p->total_rows == 0) return 0;
+  HSTU_CHECK_ARG(operands != nullptr && (reinterpret_cast<uintptr_t>(operands) & 255) == 0,
+                 "operands must be a 256-byte aligned buffer (got %p)", operands);
+  if (int e = bind_device(p->q)) return e;
+  if (!runs_on_fp16_operands(p, false)) {
+    set_error("hstu_attn_fwd_keep_fp16_operands: only bf16 at dqk == dv == 32 on the wgmma kernels runs on fp16 operands");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  const size_t need = fp16_operands_workspace_bytes(*p, false);
+  HSTU_CHECK_ARG(operands_bytes >= need, "operands buffer of %zu bytes required (got %zu)", need, operands_bytes);
+  hstu_attn_params c = *p;  // the operands buffer has the layout of the forward's workspace
+  c.workspace = operands;
+  c.workspace_bytes = need;
+  return attn_wgmma_fwd(c, (cudaStream_t)stream);
+}
+
+size_t hstu_attn_bwd_fp16_operands_workspace_bytes(const hstu_attn_params* p) {
+  if (p == nullptr || p->batch <= 0 || p->heads <= 0 || p->total_rows <= 0) return 0;
+  return fp16_operands_dout_workspace_bytes(*p);
+}
+
+int hstu_attn_bwd_on_fp16_operands(const hstu_attn_params* p, const void* operands, size_t operands_bytes, void* stream) {
+  HSTU_CHECK_ARG(p != nullptr, "params is NULL");
+  HSTU_CHECK_ARG(operands != nullptr && (reinterpret_cast<uintptr_t>(operands) & 255) == 0,
+                 "operands must be a 256-byte aligned buffer (got %p)", operands);
+  // q, k, v: the copies in the buffer, contiguous [L, H, 32] views, so that every check sees the tensors the kernels read
+  hstu_attn_params c = *p;
+  const Fp16Operands kept = fp16_operands_at(c, const_cast<void*>(operands));
+  c.q = kept.copy[0], c.k = kept.copy[1], c.v = kept.copy[2];
+  c.q_row_stride = c.k_row_stride = c.v_row_stride = (int64_t)c.heads * c.dqk;
+  c.q_head_stride = c.k_head_stride = c.v_head_stride = c.dqk;
+  if (int e = validate_attn(&c, true)) return e;
+  if (c.batch == 0 || c.total_rows == 0) return 0;
+  // a buffer kept for other sizes (batch, heads, rows) would be read out of bounds
+  const size_t need = fp16_operands_workspace_bytes(c, false);
+  HSTU_CHECK_ARG(operands_bytes >= need, "operands buffer of %zu bytes required (got %zu): not kept by a forward of these sizes",
+                 need, operands_bytes);
+  if (int e = bind_device(c.dout)) return e;
+  if (!runs_on_fp16_operands(&c, true)) {
+    set_error("hstu_attn_bwd_on_fp16_operands: only bf16 at dqk == dv == 32 on the wgmma kernels runs on fp16 operands");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  return attn_wgmma_bwd_on_fp16_operands(c, operands, (cudaStream_t)stream);
 }
 
 int hstu_mask_valid(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,

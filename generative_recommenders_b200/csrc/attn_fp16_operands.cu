@@ -5,6 +5,10 @@
 // Both run one CTA per (256-row block, head, sequence) over the rows < max_seq_len of each sequence.  Rows of the copies
 // past max_seq_len are not written: the attention kernels treat them as rows past the sequence end, which never reach an
 // MMA (zero_tile_rows, DESIGN.md 2).
+// The forward's workspace, [B, H, 4] amax bits then the q, k, v copies, is also the layout of the operands buffer that
+// hstu_attn_fwd_keep_fp16_operands leaves to the caller.  hstu_attn_bwd_on_fp16_operands reads q, k, v and their amax from
+// that buffer and runs both kernels over dO alone, into its own workspace: the amax block copied from the buffer (its dO
+// slots are zero there), then the dO copy.  Its q, k, v exponents are then the forward's, and so are the bits of the copies.
 // The fp8 forward (attn_wgmma_fwd_e4m3.cu) reuses the convert kernel to widen its e4m3 v to fp16, [L, H, dv]: every finite
 // e4m3 value is a normal fp16 value, so that copy is exact and needs no scale (and no amax pass).
 #include <cuda_fp16.h>
@@ -27,7 +31,8 @@ struct PreOperand {
 
 struct PreParams {
   PreOperand op[kAmaxSlots];
-  int nops;  // 3 (q, k, v) or 4 (+ dO)
+  int nops;   // 3 (q, k, v), 4 (+ dO), or 1 (dO alone, or the fp8 forward's v)
+  int slot0;  // amax slot of op[0]: kAmaxQ, or kAmaxDO for dO alone
   const void* seq_offsets;
   int offsets_i64, max_seq_len, heads;
   int d;  // columns of the e4m3 operand (the bf16 operands have kPreD)
@@ -71,7 +76,7 @@ __global__ void __launch_bounds__(kPreThreads) fp16_operands_amax_kernel(const _
     uint32_t m = 0u;
 #pragma unroll
     for (int w = 0; w < kPreThreads / 32; ++w) m = max(m, red[threadIdx.x][w]);
-    if (m) atomicMax(p.amax + ((long long)b * p.heads + h) * kAmaxSlots + threadIdx.x, m);
+    if (m) atomicMax(p.amax + ((long long)b * p.heads + h) * kAmaxSlots + p.slot0 + threadIdx.x, m);
   }
 }
 
@@ -93,7 +98,7 @@ __global__ void __launch_bounds__(kPreThreads) fp16_operands_convert_kernel(cons
   }
   for (int o = 0; o < p.nops; ++o) {
     const PreOperand& op = p.op[o];
-    const int e = exps[o];
+    const int e = exps[p.slot0 + o];
     for (int c = threadIdx.x; c < rows * cpr; c += kPreThreads) {
       const int r = c / cpr, part = c % cpr;
       const long long row = row0 + r0 + r;
@@ -128,11 +133,37 @@ __global__ void __launch_bounds__(kPreThreads) fp16_operands_convert_kernel(cons
 // host
 // ------------------------------------------------------------------------------------------------
 static size_t align256(size_t n) { return (n + 255) / 256 * 256; }
+static size_t amax_bytes(const hstu_attn_params& p) { return (size_t)p.batch * p.heads * kAmaxSlots * sizeof(uint32_t); }
+static size_t copy_bytes(const hstu_attn_params& p) { return align256((size_t)p.total_rows * p.heads * kPreD * sizeof(__half)); }
 
 size_t fp16_operands_workspace_bytes(const hstu_attn_params& p, bool bwd) {
-  const size_t amax = align256((size_t)p.batch * p.heads * kAmaxSlots * sizeof(uint32_t));
-  const size_t copy = align256((size_t)p.total_rows * p.heads * kPreD * sizeof(__half));
-  return amax + (bwd ? 4 : 3) * copy;
+  return align256(amax_bytes(p)) + (bwd ? 4 : 3) * copy_bytes(p);
+}
+
+size_t fp16_operands_dout_workspace_bytes(const hstu_attn_params& p) { return align256(amax_bytes(p)) + copy_bytes(p); }
+
+Fp16Operands fp16_operands_at(const hstu_attn_params& p, void* buf) {
+  uint8_t* base = reinterpret_cast<uint8_t*>(buf);
+  Fp16Operands f;
+  f.amax = reinterpret_cast<uint32_t*>(base);
+  for (int o = 0; o < kAmaxSlots; ++o) f.copy[o] = base + align256(amax_bytes(p)) + o * copy_bytes(p);
+  return f;
+}
+
+// Both kernels over pp.op[0 .. pp.nops), into pp.amax (zeroed, or holding the amax of the other operands) and pp.op[].dst
+static int launch_prepass(const hstu_attn_params& p, PreParams& pp, cudaStream_t st) {
+  pp.seq_offsets = p.seq_offsets;
+  pp.offsets_i64 = p.offsets_are_i64;
+  pp.max_seq_len = p.max_seq_len;
+  pp.heads = p.heads;
+  pp.alpha = p.alpha;
+  if (p.batch == 0 || p.max_seq_len <= 0) return 0;
+  const dim3 grid((p.max_seq_len + kPreRows - 1) / kPreRows, p.heads, p.batch);
+  fp16_operands_amax_kernel<<<grid, kPreThreads, 0, st>>>(pp);
+  HSTU_CUDA_OK(cudaGetLastError());
+  fp16_operands_convert_kernel<false><<<grid, kPreThreads, 0, st>>>(pp);
+  HSTU_CUDA_OK(cudaGetLastError());
+  return 0;
 }
 
 int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out, cudaStream_t st) {
@@ -141,12 +172,10 @@ int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out
     set_error("hstu_attn_%s: workspace of %zu bytes required (got %zu)", bwd ? "bwd" : "fwd", need, p.workspace_bytes);
     return HSTU_ERR_WORKSPACE;
   }
-  uint8_t* ws = reinterpret_cast<uint8_t*>(p.workspace);
-  const size_t amax_bytes = (size_t)p.batch * p.heads * kAmaxSlots * sizeof(uint32_t);
-  const size_t copy = align256((size_t)p.total_rows * p.heads * kPreD * sizeof(__half));
+  *out = fp16_operands_at(p, p.workspace);
   PreParams pp;
   memset(&pp, 0, sizeof(pp));
-  pp.amax = reinterpret_cast<uint32_t*>(ws);
+  pp.amax = const_cast<uint32_t*>(out->amax);
   const void* src[kAmaxSlots] = {p.q, p.k, p.v, p.dout};
   const long long rs[kAmaxSlots] = {p.q_row_stride, p.k_row_stride, p.v_row_stride, p.do_row_stride};
   const long long hs[kAmaxSlots] = {p.q_head_stride, p.k_head_stride, p.v_head_stride, p.do_head_stride};
@@ -155,23 +184,33 @@ int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out
     pp.op[o].src = src[o];
     pp.op[o].row_stride = rs[o];
     pp.op[o].head_stride = hs[o];
-    pp.op[o].dst = reinterpret_cast<__half*>(ws + align256(amax_bytes) + o * copy);
-    out->copy[o] = pp.op[o].dst;
+    pp.op[o].dst = reinterpret_cast<__half*>(const_cast<void*>(out->copy[o]));
   }
-  out->amax = pp.amax;
-  pp.seq_offsets = p.seq_offsets;
-  pp.offsets_i64 = p.offsets_are_i64;
-  pp.max_seq_len = p.max_seq_len;
-  pp.heads = p.heads;
-  pp.alpha = p.alpha;
-  HSTU_CUDA_OK(cudaMemsetAsync(pp.amax, 0, amax_bytes, st));
-  if (p.batch == 0 || p.max_seq_len <= 0) return 0;
-  const dim3 grid((p.max_seq_len + kPreRows - 1) / kPreRows, p.heads, p.batch);
-  fp16_operands_amax_kernel<<<grid, kPreThreads, 0, st>>>(pp);
-  HSTU_CUDA_OK(cudaGetLastError());
-  fp16_operands_convert_kernel<false><<<grid, kPreThreads, 0, st>>>(pp);
-  HSTU_CUDA_OK(cudaGetLastError());
-  return 0;
+  HSTU_CUDA_OK(cudaMemsetAsync(pp.amax, 0, amax_bytes(p), st));
+  return launch_prepass(p, pp, st);
+}
+
+int fp16_operands_dout_prepass(const hstu_attn_params& p, const void* kept, Fp16Operands* out, cudaStream_t st) {
+  const size_t need = fp16_operands_dout_workspace_bytes(p);
+  if (p.workspace == nullptr || p.workspace_bytes < need) {
+    set_error("hstu_attn_bwd_on_fp16_operands: workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
+    return HSTU_ERR_WORKSPACE;
+  }
+  const Fp16Operands k = fp16_operands_at(p, const_cast<void*>(kept)), w = fp16_operands_at(p, p.workspace);
+  out->amax = w.amax;
+  for (int o = 0; o < 3; ++o) out->copy[o] = k.copy[o];
+  out->copy[kAmaxDO] = w.copy[0];  // the only copy of the workspace
+  PreParams pp;
+  memset(&pp, 0, sizeof(pp));
+  pp.amax = const_cast<uint32_t*>(w.amax);
+  pp.nops = 1;
+  pp.slot0 = kAmaxDO;
+  pp.op[0].src = p.dout;
+  pp.op[0].row_stride = p.do_row_stride;
+  pp.op[0].head_stride = p.do_head_stride;
+  pp.op[0].dst = reinterpret_cast<__half*>(const_cast<void*>(w.copy[0]));
+  HSTU_CUDA_OK(cudaMemcpyAsync(pp.amax, k.amax, amax_bytes(p), cudaMemcpyDeviceToDevice, st));
+  return launch_prepass(p, pp, st);
 }
 
 size_t e4m3_v_copy_bytes(const hstu_attn_params& p) { return align256((size_t)p.total_rows * p.heads * p.dv * sizeof(__half)); }

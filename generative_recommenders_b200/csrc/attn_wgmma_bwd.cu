@@ -140,4 +140,10 @@ int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st) {
   return HSTU_ERR_UNSUPPORTED;
 }
 
+int attn_wgmma_bwd_on_fp16_operands(const hstu_attn_params& p, const void* kept, cudaStream_t st) {
+  Fp16Operands f16;
+  if (int e = fp16_operands_dout_prepass(p, kept, &f16, st)) return e;
+  return launch_bwd_wgmma<32, false, true>(p, st, &f16);
+}
+
 }  // namespace hstu

@@ -17,6 +17,8 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd);
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
+// attn_wgmma_bwd.cu: the bf16 d = 32 backward on the fp16 operands a forward kept (hstu_attn_bwd_on_fp16_operands)
+int attn_wgmma_bwd_on_fp16_operands(const hstu_attn_params& p, const void* kept, cudaStream_t st);
 // attn_wgmma_mixed_fwd.cu / attn_wgmma_mixed_bwd.cu: the same at dqk < dv (both in {32, 64, 128, 256})
 int attn_wgmma_fwd_mixed(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd_mixed(const hstu_attn_params& p, cudaStream_t st);
@@ -33,7 +35,14 @@ struct Fp16Operands {
   const void* copy[4];       // fp16 [L, H, 32] copies of q, k, v, dO (dO: backward only)
 };
 size_t fp16_operands_workspace_bytes(const hstu_attn_params& p, bool bwd);
+// the amax block at the start of `buf` (a workspace, or the operands buffer of a kept-operands call) and the copies after it
+// (as many as `buf` holds)
+Fp16Operands fp16_operands_at(const hstu_attn_params& p, void* buf);
 int fp16_operands_prepass(const hstu_attn_params& p, bool bwd, Fp16Operands* out, cudaStream_t st);
+// the backward on operands a forward kept (hstu_attn_bwd_on_fp16_operands): q, k, v and their amax from `kept`, dO's amax
+// and copy into the workspace
+size_t fp16_operands_dout_workspace_bytes(const hstu_attn_params& p);
+int fp16_operands_dout_prepass(const hstu_attn_params& p, const void* kept, Fp16Operands* out, cudaStream_t st);
 // the fp8 forward's fp16 copy of the e4m3 v, [L, H, dv] contiguous (exact: no scale), at the start of the workspace
 size_t e4m3_v_copy_bytes(const hstu_attn_params& p);
 int e4m3_v_prepass(const hstu_attn_params& p, const void** v16, cudaStream_t st);

@@ -60,15 +60,36 @@ def _prep(*ts):
     return tuple(switch_to_contiguous_if_needed(t) for t in ts)
 
 
+def _wgmma_view(t: torch.Tensor) -> torch.Tensor:
+    """t, or a contiguous copy of it where the wgmma kernels could not take it (a 16-byte base, row / head strides of whole
+    16-byte units)."""
+    ok = t.data_ptr() % 16 == 0 and t.stride(0) % 8 == 0 and t.stride(1) % 8 == 0
+    return t if ok else t.clone(memory_format=torch.contiguous_format)
+
+
+class Fp16Operands:
+    """The scaled fp16 copies of q, k, v and their per (sequence, head) amax that a bf16 attention at dqk == dv == 32 runs on
+    (include/hstu_b200.h, hstu_attn_fwd_keep_fp16_operands).  Pass an empty one to `cuda_hstu_attention_fwd` and the same one
+    to the backward of the same q, k, v: the forward fills it, and the backward then converts dO alone and reads neither q,
+    k nor v.  A forward that does not run on such operands leaves it empty, and the backward then takes q, k, v as usual."""
+
+    def __init__(self):
+        self.buf: Optional[torch.Tensor] = None  # uint8, the library's layout from a 256-byte aligned `base`
+        self.base = 0
+        self.nbytes = 0  # from `base`: the backward checks it against what its sizes need
+
+
 def cuda_hstu_attention_fwd(
     max_seq_len: int, alpha: float, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, seq_offsets: torch.Tensor,
     num_targets: Optional[torch.Tensor] = None, max_attn_len: int = 0, contextual_seq_len: int = 0,
     min_full_attn_seq_len: int = 0, impl: int = _lib.IMPL_AUTO, delta_q_len: int = 0,
     out: Optional[torch.Tensor] = None, bias: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
     descales: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor], Optional[torch.Tensor]]] = None,
+    fp16_operands: Optional[Fp16Operands] = None,
 ) -> torch.Tensor:
     """descales: (q_descale, k_descale, v_descale) of fp8 inputs -- see cuda_hstu_attention_fwd_fp8.  q, k, v of dtype
-    torch.float8_e4m3fn take that path with or without descales."""
+    torch.float8_e4m3fn take that path with or without descales.  fp16_operands: an empty Fp16Operands that keeps the
+    call's fp16 operands for its backward, if it runs on them."""
     if descales is not None or any(t.dtype == _FP8 for t in (q, k, v)):
         if bias is not None or delta_q_len:
             raise RuntimeError("fp8 attention: the relative bias and delta_q are not supported")
@@ -87,13 +108,23 @@ def cuda_hstu_attention_fwd(
     p.out = out.data_ptr()
     p.o_row_stride, p.o_head_stride = out.stride(0), out.stride(1)
     keep = _fill_bias(p, bias, None)
-    ws = _workspace(p, False, dev)
-    with torch.cuda.device(dev), _lib.timed("attn_fwd", dev):
-        _lib.check(_lib.lib().hstu_attn_fwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_fwd")
+    kept = _lib.lib().hstu_attn_fp16_operands_bytes(C.byref(p)) if fp16_operands is not None else 0
+    if kept:
+        fp16_operands.buf = torch.empty(kept + 256, dtype=torch.uint8, device=dev)
+        fp16_operands.base = (fp16_operands.buf.data_ptr() + 255) // 256 * 256
+        fp16_operands.nbytes = kept
+        ws = None  # the pre-pass writes into the operands buffer instead of a workspace
+        with torch.cuda.device(dev), _lib.timed("attn_fwd", dev):
+            _lib.check(_lib.lib().hstu_attn_fwd_keep_fp16_operands(C.byref(p), fp16_operands.base, kept, _lib.stream_ptr(dev)),
+                       "hstu_attn_fwd_keep_fp16_operands")
+    else:
+        ws = _workspace(p, False, dev)
+        with torch.cuda.device(dev), _lib.timed("attn_fwd", dev):
+            _lib.check(_lib.lib().hstu_attn_fwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_fwd")
     if delta_q_len:  # a workspace holds the partials of split key chunks: the attention kernel, then their reduction
         _lib.note_launch(2 if ws is not None else 1)
-    else:  # bf16 at d = 32: amax and convert kernels before the attention kernel (the workspace: the fp16 copies)
-        _lib.note_launch(3 if ws is not None else 1)
+    else:  # bf16 at d = 32: amax and convert kernels before the attention kernel (into the workspace or the operands buffer)
+        _lib.note_launch(3 if ws is not None or kept else 1)
     del ws, keep
     return out
 
@@ -158,8 +189,13 @@ def cuda_hstu_attention_bwd(
     bias: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
     dbias: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
     deterministic: Optional[bool] = None,
+    fp16_operands: Optional[Fp16Operands] = None,
 ) -> None:
     """Writes dq, dk, dv in place (last-dim stride 1 required; row/head strides arbitrary).
+
+    fp16_operands: what the forward of these q, k, v kept (Fp16Operands).  If it holds operands, q, k, v are not read and may
+    be None; that backward runs on the wgmma kernels only, so a dout or dq / dk / dv view they cannot take goes through a
+    contiguous copy.
 
     deterministic: dq / dk / dv bitwise reproducible from run to run (the wgmma backward then runs its atomic-free dK / dV
     and dQ kernels at every head dim); None follows torch.are_deterministic_algorithms_enabled().  Not available with a
@@ -167,11 +203,18 @@ def cuda_hstu_attention_bwd(
     """
     if deterministic is None:
         deterministic = torch.are_deterministic_algorithms_enabled()
+    kept = fp16_operands is not None and fp16_operands.buf is not None
+    if kept and q is None:  # dqk == dv: dout has the shape and dtype of q, k and v
+        q = k = v = dout
     dev = _lib.require_cuda(dout, q, k, v, dq, dk, dv, seq_offsets, num_targets)
     q, k, v, dout = _prep(q, k, v, dout)
     for g in (dq, dk, dv):
         if g.stride(-1) != 1:
             raise RuntimeError("dq/dk/dv must have a dense last dimension")
+    grads = (dq, dk, dv)
+    if kept:  # no generic fallback without q, k, v
+        dout = _wgmma_view(dout)
+        dq, dk, dv = (_wgmma_view(g) for g in grads)
     seq_offsets = seq_offsets.contiguous()
     if num_targets is not None:
         num_targets = num_targets.contiguous()
@@ -185,6 +228,20 @@ def cuda_hstu_attention_bwd(
     p.dv_row_stride, p.dv_head_stride = dv.stride(0), dv.stride(1)
     p.deterministic = int(bool(deterministic))
     keep = _fill_bias(p, bias, dbias)
+    if kept:  # the amax and convert kernels over dO alone, then the dK/dV and dQ kernels
+        p.q = p.k = p.v = None
+        nbytes = _lib.lib().hstu_attn_bwd_fp16_operands_workspace_bytes(C.byref(p))
+        ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+        p.workspace, p.workspace_bytes = (ws.data_ptr() + 255) // 256 * 256, nbytes
+        with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
+            _lib.check(_lib.lib().hstu_attn_bwd_on_fp16_operands(C.byref(p), fp16_operands.base, fp16_operands.nbytes,
+                                                                 _lib.stream_ptr(dev)), "hstu_attn_bwd_on_fp16_operands")
+        _lib.note_launch(4)
+        for g, w in zip(grads, (dq, dk, dv)):
+            if w is not g:
+                g.copy_(w)
+        del ws, keep
+        return
     ws = _workspace(p, True, dev)
     with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
         _lib.check(_lib.lib().hstu_attn_bwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_bwd")
@@ -231,6 +288,8 @@ class _HSTUAttentionFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
                 min_full_attn_seq_len, impl):
+        # no Fp16Operands here: q, k, v are saved anyway, so the copies would double the saved bytes to spare only the
+        # backward's pre-pass over q, k, v
         out = cuda_hstu_attention_fwd(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
                                       contextual_seq_len, min_full_attn_seq_len, impl)
         ctx.save_for_backward(q, k, v, seq_offsets, num_targets)

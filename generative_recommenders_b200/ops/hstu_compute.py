@@ -14,7 +14,7 @@ import torch
 
 from .. import _lib
 from ..common import HammerKernel, require_cuda_kernel
-from .hstu_attention import cuda_hstu_attention_bwd, cuda_hstu_attention_fwd, hstu_mha
+from .hstu_attention import Fp16Operands, cuda_hstu_attention_bwd, cuda_hstu_attention_fwd, hstu_mha
 from .layer_norm import _partial, cuda_layer_norm_bwd, cuda_layer_norm_fwd, layer_norm
 
 
@@ -191,8 +191,13 @@ class _HSTUPreprocessAndAttentionFunction(torch.autograd.Function):
         H, dqk, dv = num_heads, attn_dim, hidden_dim
         u_pre, v, q, k = torch.split(uvqk, [dv * H, dv * H, dqk * H, dqk * H], dim=1)
         u = cuda_silu_fwd(u_pre)
+        # bf16 at dqk == dv == 32: the attention keeps its fp16 copies of q, k, v for the backward, which then needs only u
+        # of the uvqk GEMM (L * H * 32 * 2 bytes per copy: memory traded for the q / k / v columns of the recomputed GEMM
+        # and the backward's pre-pass over them)
+        ops = Fp16Operands()
         out = cuda_hstu_attention_fwd(max_seq_len, attn_alpha, q.view(-1, H, dqk), k.view(-1, H, dqk), v.view(-1, H, dv),
-                                      seq_offsets, num_targets, max_attn_len, contextual_seq_len, 0, impl)
+                                      seq_offsets, num_targets, max_attn_len, contextual_seq_len, 0, impl, fp16_operands=ops)
+        ctx.fp16_operands = ops
         ctx.save_for_backward(x, norm_weight, norm_bias, uvqk_weight, uvqk_bias, mean, rstd, seq_offsets, num_targets,
                               None if recompute_normed_x else normed_x,
                               None if recompute_uvqk else uvqk)
@@ -204,17 +209,23 @@ class _HSTUPreprocessAndAttentionFunction(torch.autograd.Function):
         (x, norm_weight, norm_bias, uvqk_weight, uvqk_bias, mean, rstd, seq_offsets, num_targets, normed_x,
          uvqk) = ctx.saved_tensors
         norm_eps, H, dqk, dv, max_seq_len, alpha, max_attn_len, contextual_seq_len, impl = ctx.cfg
+        ops = ctx.fp16_operands
         if normed_x is None:
             normed_x, _, _ = cuda_layer_norm_fwd(x, norm_weight, norm_bias, norm_eps, False, save_stats=False)
-        if uvqk is None:
-            uvqk = torch.addmm(uvqk_bias, normed_x, uvqk_weight)
-        u_pre, v, q, k = torch.split(uvqk, [dv * H, dv * H, dqk * H, dqk * H], dim=1)
-        duvqk = torch.empty_like(uvqk)
+        if uvqk is None and ops.buf is not None:  # the attention reads the forward's fp16 q, k, v: the u columns only
+            u_pre = torch.addmm(uvqk_bias[:dv * H], normed_x, uvqk_weight[:, :dv * H])
+            q = k = v = None
+        else:
+            if uvqk is None:
+                uvqk = torch.addmm(uvqk_bias, normed_x, uvqk_weight)
+            u_pre, v, q, k = torch.split(uvqk, [dv * H, dv * H, dqk * H, dqk * H], dim=1)
+            q, k, v = q.view(-1, H, dqk), k.view(-1, H, dqk), v.view(-1, H, dv)
+        duvqk = torch.empty((normed_x.shape[0], uvqk_weight.shape[1]), dtype=normed_x.dtype, device=normed_x.device)
         d_u, d_v, d_q, d_k = torch.split(duvqk, [dv * H, dv * H, dqk * H, dqk * H], dim=1)
         dattn = _row_major(dattn)
-        cuda_hstu_attention_bwd(max_seq_len, alpha, dattn.view(-1, H, dv), q.view(-1, H, dqk), k.view(-1, H, dqk),
-                                v.view(-1, H, dv), d_q.view(-1, H, dqk), d_k.view(-1, H, dqk), d_v.view(-1, H, dv),
-                                seq_offsets, num_targets, max_attn_len, contextual_seq_len, 0, impl)
+        cuda_hstu_attention_bwd(max_seq_len, alpha, dattn.view(-1, H, dv), q, k, v, d_q.view(-1, H, dqk), d_k.view(-1, H, dqk),
+                                d_v.view(-1, H, dv), seq_offsets, num_targets, max_attn_len, contextual_seq_len, 0, impl,
+                                fp16_operands=ops)
         cuda_silu_bwd(du, u_pre, d_u)
         d_w = torch.mm(normed_x.t(), duvqk)
         d_b = duvqk.sum(dim=0)

@@ -129,6 +129,26 @@ size_t hstu_attn_workspace_bytes(const hstu_attn_params* p, int is_backward);
 int hstu_attn_fwd(const hstu_attn_params* p, void* cuda_stream);
 int hstu_attn_bwd(const hstu_attn_params* p, void* cuda_stream);
 
+/* A bf16 attention at dqk == dv == 32 runs on the wgmma kernels on exactly scaled fp16 copies of q, k, v (and dO) with their
+ * per (sequence, head) amax, which a pre-pass writes before each call.  A forward can leave its copies to the caller, and
+ * the backward of the same q, k, v (same seq_offsets, max_seq_len and alpha) can then take them instead: it scales and
+ * converts dO alone.  dq, dk, dv are bitwise those of hstu_attn_bwd.
+ * hstu_attn_fp16_operands_bytes: bytes of the caller's operands buffer ([B, H, 4] amax bits, then the fp16 copies of q, k
+ * and v, [L, H, 32] each), or 0 if the call does not run on such operands (another dtype or head dim, delta_q, a relative
+ * bias, the generic kernels) or is empty.
+ * hstu_attn_fwd_keep_fp16_operands: hstu_attn_fwd writing them into `operands` (operands_bytes >= that many, 256-byte
+ * aligned); it uses no workspace.  HSTU_ERR_UNSUPPORTED where hstu_attn_fp16_operands_bytes is 0.
+ * hstu_attn_bwd_on_fp16_operands: hstu_attn_bwd on such a buffer of operands_bytes bytes, unchanged since its forward
+ * (HSTU_ERR_INVALID_ARGUMENT if it is smaller than these sizes need); q, k, v and their strides are not read (they may be
+ * NULL / 0).  dout, dq, dk, dv must be views the wgmma backward takes (16-byte base, row / head strides of whole 16-byte
+ * units): there is no generic fallback without q, k, v.  Its workspace: hstu_attn_bwd_fp16_operands_workspace_bytes(p)
+ * bytes (dO's amax and copy; sizes only). */
+size_t hstu_attn_fp16_operands_bytes(const hstu_attn_params* p);
+int hstu_attn_fwd_keep_fp16_operands(const hstu_attn_params* p, void* operands, size_t operands_bytes, void* cuda_stream);
+size_t hstu_attn_bwd_fp16_operands_workspace_bytes(const hstu_attn_params* p);
+int hstu_attn_bwd_on_fp16_operands(const hstu_attn_params* p, const void* operands, size_t operands_bytes,
+                                   void* cuda_stream);
+
 /* Per (sequence, head) dequantisation scales of the fp8 forward.  Each pointer is an fp32 device array read at
  * [b * batch_stride + h * head_stride] (strides in elements, >= 0), or NULL for a scale of 1. */
 typedef struct hstu_attn_descales {
