@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle import hstu_oracle as O
-from util import TOL, assert_rel, assert_same_zeros
+from util import TOL, _assert_ulp, assert_rel, assert_same_zeros
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -251,30 +251,6 @@ def test_dropout_group_norm_scalar_path_matches_layer_norm_view():
 # ------------------------------------------------------------------------------------------------------------------
 # SiLU on a strided column block
 # ------------------------------------------------------------------------------------------------------------------
-_BITS = {torch.float32: (23, -126), torch.bfloat16: (7, -126), torch.float16: (10, -14)}  # fraction bits, min normal exponent
-
-
-def _ulp(r, dtype):
-    """Spacing of `dtype` at the (fp64) values r, which are representable in dtype."""
-    p, emin = _BITS[dtype]
-    e = torch.floor(torch.log2(r.abs().clamp_min(2.0 ** emin))).clamp_min(emin)
-    return torch.exp2(e - p)
-
-
-def _assert_ulp(got, ref64, mag, dtype, what):
-    """got within 1 ulp of dtype of the fp64 value rounded to dtype, plus the error of the fp32 evaluation itself: the kernel
-    uses __expf (at most 2 + 1.173 |x| ulp) and __fdividef (2 ulp) and a few more roundings, so (10 + 1.2 |x|) fp32 ulp of the
-    magnitude `mag` of the unrounded terms.  That second part is far below one bf16 / fp16 ulp except where the result
-    cancels to nearly zero; in fp32 it is the whole bound."""
-    r = ref64.to(dtype).double()
-    x_abs = mag[1]
-    lim = _ulp(r, dtype) + (10 + 1.2 * x_abs) * 2.0 ** -23 * mag[0]
-    err = (got.double().cpu() - r).abs()
-    bad = ~(err <= lim)
-    assert not bad.any(), (f"{what}: {int(bad.sum())} elements beyond 1 ulp; first at {tuple(int(i) for i in bad.nonzero()[0])}: "
-                           f"got {float(got.double().cpu()[bad][0]):.8e}, ref {float(ref64[bad][0]):.8e}")
-
-
 def _silu_refs(x, dy):
     x64, dy64 = x.double().cpu(), dy.double().cpu()
     sg = torch.sigmoid(x64)

@@ -92,6 +92,50 @@ def assert_rel_segments(actual: torch.Tensor, ref: torch.Tensor, seq_offsets, ma
     return max((x[0] for x in segs), default=0.0)
 
 
+BLOCK_ROWS = 4224  # rows of one pass of the length-256 output-stage backward: 528 CTAs x 8 warps, one row per warp each
+
+
+def rel_row_sums(actual: torch.Tensor, ref: torch.Tensor) -> torch.Tensor:
+    """[n, 4] fp64 per-row sums of two [n, W] tensors: squared error, squared reference, squared storage rounding of the
+    reference in actual.dtype, and the element count.  Sums of row chunks concatenate, so a check of a tensor too large for
+    host memory can be assembled chunk by chunk."""
+    a = actual.detach().cpu().double().reshape(actual.shape[0], -1)
+    r = ref.detach().cpu().double().reshape(ref.shape[0], -1)
+    q = torch.zeros_like(r) if actual.dtype == torch.float32 else r.to(actual.dtype).double() - r
+    cnt = torch.full((r.shape[0],), float(r.shape[1]), dtype=torch.float64)
+    return torch.stack([(a - r).square().sum(1), r.square().sum(1), q.square().sum(1), cnt], 1)
+
+
+def assert_rel_row_sums(sums: torch.Tensor, dtype: torch.dtype, what: str, block: int = BLOCK_ROWS,
+                        tol: float = None) -> float:
+    """The bound of assert_rel, sqrt(tol^2 + q^2) with q the storage rounding of `dtype` measured on the reference, on the
+    whole tensor and on every block of `block` rows, from the per-row sums of rel_row_sums.  So an error confined to one pass
+    of a persistent kernel's grid cannot hide in the rest.  A last block of fewer than SEG_MIN_ELEMS elements joins the one
+    before it.  The failure names the worst block.  Returns the largest rel-L2 of a block."""
+    t = TOL[dtype] if tol is None else tol
+    n = sums.shape[0]
+    bounds = list(range(0, n, block)) + [n]
+    if len(bounds) > 2 and float(sums[bounds[-2]:, 3].sum()) < SEG_MIN_ELEMS:
+        bounds.pop(-2)
+    segs = []
+    for r0, r1 in [(0, n)] + list(zip(bounds[:-1], bounds[1:])):
+        e2, r2, q2, _ = (float(x) for x in sums[r0:r1].sum(0))
+        den = r2 if r2 > 0 else 1.0
+        err, q = math.sqrt(e2 / den), math.sqrt(q2 / den)
+        segs.append((err, math.sqrt(t * t + q * q), q, "all rows" if (r0, r1) == (0, n) else f"rows [{r0}, {r1})"))
+    over = [x for x in segs if not x[0] <= x[1]]  # NaN counts as over
+    if over:
+        err, lim, q, label = max(over, key=lambda x: x[0] / x[1] if x[0] == x[0] else math.inf)
+        raise AssertionError(f"{what}: {label}: rel-L2 error {err:.3e} > {lim:.3e} (tol {t:.1e}, storage rounding "
+                             f"{q:.2e}); {len(over)} of {len(segs)} checks over their bound")
+    return max(x[0] for x in segs[1:])
+
+
+def assert_rel_blocks(actual: torch.Tensor, ref: torch.Tensor, what: str, block: int = BLOCK_ROWS, tol: float = None) -> float:
+    """assert_rel on the whole of an [n, W] tensor and on every block of `block` rows (assert_rel_row_sums)."""
+    return assert_rel_row_sums(rel_row_sums(actual, ref), actual.dtype, what, block, tol)
+
+
 def assert_finite_rows(t: torch.Tensor, seq_offsets, skip, what: str) -> None:
     """Every row of every sequence not in `skip` is finite; the message names the first sequence and row that is not."""
     off = [int(x) for x in torch.as_tensor(seq_offsets).cpu().tolist()]
@@ -104,6 +148,29 @@ def assert_finite_rows(t: torch.Tensor, seq_offsets, skip, what: str) -> None:
 
 
 U32 = 2.0 ** -24  # unit roundoff of fp32
+
+_BITS = {torch.float32: (23, -126), torch.bfloat16: (7, -126), torch.float16: (10, -14)}  # fraction bits, min normal exponent
+
+
+def _ulp(r, dtype):
+    """Spacing of `dtype` at the (fp64) values r, which are representable in dtype."""
+    p, emin = _BITS[dtype]
+    e = torch.floor(torch.log2(r.abs().clamp_min(2.0 ** emin))).clamp_min(emin)
+    return torch.exp2(e - p)
+
+
+def _assert_ulp(got, ref64, mag, dtype, what):
+    """got within 1 ulp of dtype of the fp64 value rounded to dtype, plus the error of the fp32 evaluation itself: the kernel
+    uses __expf (at most 2 + 1.173 |x| ulp) and __fdividef (2 ulp) and a few more roundings, so (10 + 1.2 |x|) fp32 ulp of the
+    magnitude `mag` of the unrounded terms.  That second part is far below one bf16 / fp16 ulp except where the result
+    cancels to nearly zero; in fp32 it is the whole bound."""
+    r = ref64.to(dtype).double()
+    x_abs = mag[1]
+    lim = _ulp(r, dtype) + (10 + 1.2 * x_abs) * 2.0 ** -23 * mag[0]
+    err = (got.double().cpu() - r).abs()
+    bad = ~(err <= lim)
+    assert not bad.any(), (f"{what}: {int(bad.sum())} elements beyond 1 ulp; first at {tuple(int(i) for i in bad.nonzero()[0])}: "
+                           f"got {float(got.double().cpu()[bad][0]):.8e}, ref {float(ref64[bad][0]):.8e}")
 
 
 def assert_zero_from(table: torch.Tensor, start: int, what: str) -> None:
