@@ -92,9 +92,9 @@ static int select_impl(const hstu_attn_params* p, bool bwd) {
   return can ? HSTU_IMPL_UMMA : HSTU_IMPL_GENERIC;
 }
 
-// The calls that run on scaled fp16 operands (attn_fp16_operands.cu): bf16 at dqk == dv == 32 on the wgmma kernels
-static bool runs_on_fp16_operands(const hstu_attn_params* p, bool bwd) {
-  return p->dtype == HSTU_BF16 && p->dqk == 32 && p->dv == 32 && p->delta_q_len == 0 && select_impl(p, bwd) == HSTU_IMPL_UMMA;
+// The calls that run on scaled fp16 operands (attn_fp16_operands.cu): those of runs_on_fp16_operands on the wgmma kernels
+static bool wgmma_on_fp16_operands(const hstu_attn_params* p, bool bwd) {
+  return runs_on_fp16_operands(*p) && select_impl(p, bwd) == HSTU_IMPL_UMMA;
 }
 
 // Nullable descales: no negative strides, fp32-aligned pointers.
@@ -200,7 +200,7 @@ int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* desca
 
 size_t hstu_attn_fp16_operands_bytes(const hstu_attn_params* p) {
   if (p == nullptr || validate_attn(p, false) != 0) return 0;
-  if (p->batch == 0 || p->total_rows == 0 || !runs_on_fp16_operands(p, false)) return 0;
+  if (p->batch == 0 || p->total_rows == 0 || !wgmma_on_fp16_operands(p, false)) return 0;
   return fp16_operands_workspace_bytes(*p, false);
 }
 
@@ -210,7 +210,7 @@ int hstu_attn_fwd_keep_fp16_operands(const hstu_attn_params* p, void* operands, 
   HSTU_CHECK_ARG(operands != nullptr && (reinterpret_cast<uintptr_t>(operands) & 255) == 0,
                  "operands must be a 256-byte aligned buffer (got %p)", operands);
   if (int e = bind_device(p->q)) return e;
-  if (!runs_on_fp16_operands(p, false)) {
+  if (!wgmma_on_fp16_operands(p, false)) {
     set_error("hstu_attn_fwd_keep_fp16_operands: only bf16 at dqk == dv == 32 on the wgmma kernels runs on fp16 operands");
     return HSTU_ERR_UNSUPPORTED;
   }
@@ -244,7 +244,7 @@ int hstu_attn_bwd_on_fp16_operands(const hstu_attn_params* p, const void* operan
   HSTU_CHECK_ARG(operands_bytes >= need, "operands buffer of %zu bytes required (got %zu): not kept by a forward of these sizes",
                  need, operands_bytes);
   if (int e = bind_device(c.dout)) return e;
-  if (!runs_on_fp16_operands(&c, true)) {
+  if (!wgmma_on_fp16_operands(&c, true)) {
     set_error("hstu_attn_bwd_on_fp16_operands: only bf16 at dqk == dv == 32 on the wgmma kernels runs on fp16 operands");
     return HSTU_ERR_UNSUPPORTED;
   }

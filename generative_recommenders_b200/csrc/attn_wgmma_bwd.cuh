@@ -1,5 +1,5 @@
 // Jagged HSTU attention backward on the Hopper warpgroup tensor cores (wgmma) with TMA-staged tiles: the kernel bodies and
-// the launcher of the split kernels, shared by attn_wgmma_bwd.cu (dqk == dv in {32, 64, 128, 256}) and
+// their launchers (fused and split), shared by attn_wgmma_bwd.cu (dqk == dv in {32, 64, 128, 256}) and
 // attn_wgmma_mixed_bwd.cu (dqk < dv, both in that set, split kernels only).  bf16 / fp16.  Two widths: DQK, of Q, K, dQ, dK
 // and the reduction of S = Q K^T, and DV, of V, dO, dV and the reduction of dP = dO V^T; each operand is TMA boxes of its own
 // swizzle width.  Every existing instantiation is DQK == DV == d.
@@ -50,6 +50,7 @@
 #pragma once
 #include <string.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "attn_fp16_operands.cuh"
@@ -637,20 +638,7 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
 // ------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------
-// The operands the kernels read: the inputs q, k, v, dO, or their contiguous scaled fp16 copies (d = 32, bf16), and the
-// BwdParams of the call without its tensor maps
-struct BwdOperands {
-  const void* src[4];
-  long long rs[4], hs[4];  // row / head strides (elements)
-};
-inline BwdOperands bwd_operands(const hstu_attn_params& p, const Fp16Operands* f16) {
-  BwdOperands o = {{p.q, p.k, p.v, p.dout},
-                   {p.q_row_stride, p.k_row_stride, p.v_row_stride, p.do_row_stride},
-                   {p.q_head_stride, p.k_head_stride, p.v_head_stride, p.do_head_stride}};
-  if (f16)
-    for (int i = 0; i < 4; ++i) o.src[i] = f16->copy[i], o.rs[i] = (long long)p.heads * p.dqk, o.hs[i] = p.dqk;
-  return o;
-}
+// The BwdParams of a call without its tensor maps; f16: the scaled fp16 copies of bf16 inputs, or null
 inline BwdParams bwd_params(const hstu_attn_params& p, const Fp16Operands* f16) {
   BwdParams bp;
   memset(&bp, 0, sizeof(bp));
@@ -671,20 +659,52 @@ inline BwdParams bwd_params(const hstu_attn_params& p, const Fp16Operands* f16) 
   return bp;
 }
 
+// The tensor maps of q, k, v, dO for one kernel: q in boxes of q_cols x q_rows, k in k_cols x kv_rows, v in v_cols x kv_rows,
+// dO in v_cols x q_rows
+template <int DQK, int DV>
+int bwd_tmaps(BwdParams& bp, const hstu_attn_params& p, const Operands& o, int q_cols, int k_cols, int v_cols, int q_rows, int kv_rows) {
+  if (int e = make_tmap_rows_heads(&bp.tmQ, o.src[0], p.total_rows, p.heads, DQK, o.rs[0], o.hs[0], q_cols, q_rows)) return e;
+  if (int e = make_tmap_rows_heads(&bp.tmK, o.src[1], p.total_rows, p.heads, DQK, o.rs[1], o.hs[1], k_cols, kv_rows)) return e;
+  if (int e = make_tmap_rows_heads(&bp.tmV, o.src[2], p.total_rows, p.heads, DV, o.rs[2], o.hs[2], v_cols, kv_rows)) return e;
+  return make_tmap_rows_heads(&bp.tmDO, o.src[3], p.total_rows, p.heads, DV, o.rs[3], o.hs[3], v_cols, q_rows);
+}
+
+// The fused backward at dqk == dv == D: kern (an instance of bwd_key_tile<D, D, BF16, true>) adds dQ into the fp32
+// accumulator in the workspace, and convert (dq_convert_kernel<BF16>) scales it into dq
+template <int D>
+int launch_bwd_fused(const hstu_attn_params& p, cudaStream_t st, void (*kern)(BwdParams),
+                     void (*convert)(const float*, uint16_t*, long long, int, int, long long, long long, float)) {
+  using Cfg = BwdCfg<D, D, true>;
+  const size_t need = wgmma_workspace_bytes(p, true);
+  if (p.workspace == nullptr || p.workspace_bytes < need) {
+    set_error("hstu_attn_bwd: workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
+    return HSTU_ERR_WORKSPACE;
+  }
+  BwdParams bp = bwd_params(p, nullptr);
+  if (int e = bwd_tmaps<D, D>(bp, p, operands(p, nullptr), Cfg::BOX_COLS, Cfg::BOX_COLS, Cfg::BOX_COLS, Cfg::BQ, Cfg::BKV)) return e;
+  HSTU_CUDA_OK(cudaMemsetAsync(p.workspace, 0, need, st));
+  HSTU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+  dim3 grid((p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV, p.heads, p.batch);
+  kern<<<grid, kAttnThreads, Cfg::SMEM_BYTES, st>>>(bp);
+  HSTU_CUDA_OK(cudaGetLastError());
+  const long long nvec = p.total_rows * p.heads * (D / 8);
+  const long long blocks = std::min<long long>((nvec + 255) / 256, kH100Sms * 16);
+  convert<<<(int)blocks, 256, 0, st>>>(bp.dq_acc, reinterpret_cast<uint16_t*>(p.dq), p.total_rows, p.heads, D, p.dq_row_stride,
+                                       p.dq_head_stride, bp.dk_scale);
+  HSTU_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 // The split backward: kdkdv (an instance of bwd_key_tile<DQK, DV, BF16, false>), then kdq (of bwd_dq_body<DQK, DV, BF16>);
 // no atomics and no workspace.  f16: the scaled fp16 copies of bf16 inputs (the kernels are then the fp16 ones), or null
 template <int DQK, int DV, bool BF16>
 int launch_bwd_split(const hstu_attn_params& p, cudaStream_t st, void (*kdkdv)(BwdParams), void (*kdq)(BwdParams),
                      const Fp16Operands* f16 = nullptr) {
   using Cfg = BwdCfg<DQK, DV, false>;
-  const BwdOperands o = bwd_operands(p, f16);
-  const int d[4] = {DQK, DQK, DV, DV};
+  const Operands o = operands(p, f16);
   BwdParams bp = bwd_params(p, f16);
   // the dK / dV kernel: K and V of a 128-row key tile, streamed Q_j / dO_j tiles
-  if (int e = make_tmap_rows_heads(&bp.tmQ, o.src[0], p.total_rows, p.heads, d[0], o.rs[0], o.hs[0], Cfg::BOX_COLS_Q, Cfg::BQ)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmK, o.src[1], p.total_rows, p.heads, d[1], o.rs[1], o.hs[1], Cfg::BOX_COLS, Cfg::BKV)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmV, o.src[2], p.total_rows, p.heads, d[2], o.rs[2], o.hs[2], Cfg::BOX_COLS_V, Cfg::BKV)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmDO, o.src[3], p.total_rows, p.heads, d[3], o.rs[3], o.hs[3], Cfg::BOX_COLS_V, Cfg::BQ)) return e;
+  if (int e = bwd_tmaps<DQK, DV>(bp, p, o, Cfg::BOX_COLS_Q, Cfg::BOX_COLS, Cfg::BOX_COLS_V, Cfg::BQ, Cfg::BKV)) return e;
   HSTU_CUDA_OK(cudaFuncSetAttribute(kdkdv, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   // the column slices of one key tile are adjacent CTAs (they read the same K, V and query tiles)
   const int key_ctas = (p.max_seq_len + Cfg::BKV - 1) / Cfg::BKV * Cfg::NSL;
@@ -692,10 +712,7 @@ int launch_bwd_split(const hstu_attn_params& p, cudaStream_t st, void (*kdkdv)(B
   HSTU_CUDA_OK(cudaGetLastError());
   // the dQ kernel tiles 128 query rows and DqCfg::BN key rows
   using QC = DqCfg<DQK, DV>;
-  if (int e = make_tmap_rows_heads(&bp.tmQ, o.src[0], p.total_rows, p.heads, d[0], o.rs[0], o.hs[0], QC::BOX_COLS, QC::BM)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmK, o.src[1], p.total_rows, p.heads, d[1], o.rs[1], o.hs[1], QC::BOX_COLS, QC::BN)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmV, o.src[2], p.total_rows, p.heads, d[2], o.rs[2], o.hs[2], QC::BOX_COLS_V, QC::BN)) return e;
-  if (int e = make_tmap_rows_heads(&bp.tmDO, o.src[3], p.total_rows, p.heads, d[3], o.rs[3], o.hs[3], QC::BOX_COLS_V, QC::BM)) return e;
+  if (int e = bwd_tmaps<DQK, DV>(bp, p, o, QC::BOX_COLS, QC::BOX_COLS, QC::BOX_COLS_V, QC::BM, QC::BN)) return e;
   HSTU_CUDA_OK(cudaFuncSetAttribute(kdq, cudaFuncAttributeMaxDynamicSharedMemorySize, QC::SMEM_BYTES));
   kdq<<<dim3((p.max_seq_len + QC::BM - 1) / QC::BM, p.heads, p.batch), kAttnThreads, QC::SMEM_BYTES, st>>>(bp);
   HSTU_CUDA_OK(cudaGetLastError());

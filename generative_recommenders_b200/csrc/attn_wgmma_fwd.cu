@@ -41,8 +41,7 @@ __global__ void __launch_bounds__(256) delta_reduce_kernel(const float* __restri
 // H100), into at most kDeltaCtaTarget / CTAs chunks and at most ceil(N / kDeltaChunkKeys), so that no chunk of a full-length
 // sequence is shorter than 8 key tiles.  chunks * CTAs <= kDeltaCtaTarget bounds the workspace of the partials by
 // kDeltaCtaTarget * 128 rows * dv * 4 bytes: 34.6 MB at dv = 256, 4.3 MB at dv = 32.
-// The sizing constants assume the 132 SMs of an H100 SXM; on another part they only shift the balance, never the result.
-constexpr int kH100Sms = 132;
+// The sizing constants assume the 132 SMs of an H100 SXM (kH100Sms); on another part they only shift the balance, never the result.
 constexpr int kDeltaCtaTarget = 2 * kH100Sms, kDeltaChunkKeys = 512;
 constexpr int kDeltaReduceBlocks = 8 * kH100Sms;  // grid cap of delta_reduce_kernel (grid-strided: any grid is correct)
 int delta_chunks(const hstu_attn_params& p) {
@@ -71,18 +70,33 @@ bool aligned_view(const void* ptr, long long row_stride, long long head_stride) 
   return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && (row_stride % 8) == 0 && (head_stride % 8) == 0;
 }
 
-bool wgmma_fwd_supported(const hstu_attn_params& p) {
+// What the wgmma kernels need of a call in either direction: a 16-bit dtype, the head dims, no relative bias, the row limits,
+// aligned q, k, v views, and an sm_90 device
+static bool wgmma_qkv_supported(const hstu_attn_params& p) {
   if (p.dtype != HSTU_BF16 && p.dtype != HSTU_F16) return false;
-  // dqk == dv, or dqk < dv (attn_wgmma_mixed_fwd.cu), both in {32, 64, 128, 256}
-  auto dim_ok = [](int d) { return d == 32 || d == 64 || d == 128 || d == 256; };
-  if (p.dqk > p.dv || !dim_ok(p.dqk) || !dim_ok(p.dv)) return false;
+  if (!wgmma_dims(p.dqk, p.dv)) return false;
   if (p.delta_q_len < 0 || p.pos_w != nullptr || p.ts_w != nullptr) return false;
   if (p.total_rows >= (1ll << 31) - 256 || (long long)p.batch * p.delta_q_len >= (1ll << 31) - 256) return false;
   if (!aligned_view(p.q, p.q_row_stride, p.q_head_stride) || !aligned_view(p.k, p.k_row_stride, p.k_head_stride) ||
-      !aligned_view(p.v, p.v_row_stride, p.v_head_stride) || !aligned_view(p.out, p.o_row_stride, p.o_head_stride))
+      !aligned_view(p.v, p.v_row_stride, p.v_head_stride))
     return false;
   return is_sm90();
 }
+
+static bool wgmma_fwd_supported(const hstu_attn_params& p) {
+  return wgmma_qkv_supported(p) && aligned_view(p.out, p.o_row_stride, p.o_head_stride);
+}
+
+// The backward does not read out; a given one still needs a 16-byte aligned base
+static bool wgmma_bwd_supported(const hstu_attn_params& p) {
+  if (!wgmma_qkv_supported(p) || (p.out != nullptr && !aligned_view(p.out, 0, 0))) return false;
+  // d = 256 and dqk < dv run the split kernels only; a deterministic backward there stays on the generic kernels
+  if ((p.dqk == 256 || p.dqk != p.dv) && p.deterministic) return false;
+  return aligned_view(p.dout, p.do_row_stride, p.do_head_stride) && aligned_view(p.dq, p.dq_row_stride, p.dq_head_stride) &&
+         aligned_view(p.dk, p.dk_row_stride, p.dk_head_stride) && aligned_view(p.dv_out, p.dv_row_stride, p.dv_head_stride);
+}
+
+bool wgmma_supported(const hstu_attn_params& p, bool bwd) { return bwd ? wgmma_bwd_supported(p) : wgmma_fwd_supported(p); }
 
 int launch_delta_reduce(bool bf16, const float* part, void* out, long long rows, int heads, int d, int chunks,
                         long long o_row_stride, long long o_head_stride, float inv_n, cudaStream_t st) {
@@ -94,40 +108,19 @@ int launch_delta_reduce(bool bf16, const float* part, void* out, long long rows,
   return 0;
 }
 
-// dqk == dv == D.  f16: the scaled fp16 copies of bf16 inputs (the kernel is then the fp16 one), or null
-template <int D, bool BF16, bool kDelta = false>
-static int launch_fwd(const hstu_attn_params& p, cudaStream_t st, const Fp16Operands* f16 = nullptr) {
-  auto kern = [] {
-    if constexpr (kDelta) return attn_fwd_delta_wgmma_kernel<D, BF16>;
-    else return attn_fwd_wgmma_kernel<D, BF16>;
-  }();
-  return launch_fwd_wgmma<D, D, BF16, kDelta>(p, st, kern, f16);
-}
-
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st) {
   if (p.dqk != p.dv) return attn_wgmma_fwd_mixed(p, st);
-  const bool bf = p.dtype == HSTU_BF16;
-  if (p.delta_q_len > 0) {  // bf16 keeps the hi / lo P at d = 32 too: a pre-pass over the whole cache would cost more than it saves
-    switch (p.dqk) {
-      case 32: return bf ? launch_fwd<32, true, true>(p, st) : launch_fwd<32, false, true>(p, st);
-      case 64: return bf ? launch_fwd<64, true, true>(p, st) : launch_fwd<64, false, true>(p, st);
-      case 128: return bf ? launch_fwd<128, true, true>(p, st) : launch_fwd<128, false, true>(p, st);
-      case 256: return bf ? launch_fwd<256, true, true>(p, st) : launch_fwd<256, false, true>(p, st);
-    }
-  }
-  switch (p.dqk) {
-    case 32: {  // bf16: the fp16 kernel on exactly scaled copies (DESIGN.md 3.0)
-      if (!bf) return launch_fwd<32, false>(p, st);
+  return dispatch_dims(SquareDims{}, p, "wgmma forward", [&]<int D, int, bool BF16>() {
+    // bf16 keeps the hi / lo P at d = 32 too: a pre-pass over the whole cache would cost more than it saves
+    if (p.delta_q_len > 0) return launch_fwd_wgmma<D, D, BF16, true>(p, st, attn_fwd_delta_wgmma_kernel<D, BF16>);
+    if constexpr (scaled_fp16_dims(BF16, D, D)) {  // the fp16 kernel on exactly scaled copies (DESIGN.md 3.0)
       Fp16Operands f16;
       if (int e = fp16_operands_prepass(p, false, &f16, st)) return e;
-      return launch_fwd<32, false>(p, st, &f16);
+      return launch_fwd_wgmma<D, D, false, false>(p, st, attn_fwd_wgmma_kernel<D, false>, &f16);
+    } else {
+      return launch_fwd_wgmma<D, D, BF16, false>(p, st, attn_fwd_wgmma_kernel<D, BF16>);
     }
-    case 64: return bf ? launch_fwd<64, true>(p, st) : launch_fwd<64, false>(p, st);
-    case 128: return bf ? launch_fwd<128, true>(p, st) : launch_fwd<128, false>(p, st);
-    case 256: return bf ? launch_fwd<256, true>(p, st) : launch_fwd<256, false>(p, st);
-  }
-  set_error("wgmma forward: unsupported head dim %d", p.dqk);
-  return HSTU_ERR_UNSUPPORTED;
+  });
 }
 
 }  // namespace hstu

@@ -353,17 +353,11 @@ int launch_fwd_wgmma(const hstu_attn_params& p, cudaStream_t st, void (*kern)(Fw
     fp.part = reinterpret_cast<float*>(p.workspace);
   }
   const long long q_rows = kDelta ? (long long)p.batch * p.delta_q_len : p.total_rows;
-  if (f16) {  // (dqk == dv == 32 only)
-    const long long crs = (long long)p.heads * DQK, chs = DQK;  // strides of the contiguous copies
-    if (int e = make_tmap_rows_heads(&fp.tmQ, f16->copy[0], p.total_rows, p.heads, DQK, crs, chs, Cfg::BOX_COLS, Cfg::BM)) return e;
-    if (int e = make_tmap_rows_heads(&fp.tmK, f16->copy[1], p.total_rows, p.heads, DQK, crs, chs, Cfg::BOX_COLS, Cfg::BN)) return e;
-    if (int e = make_tmap_rows_heads(&fp.tmV, f16->copy[2], p.total_rows, p.heads, DV, crs, chs, Cfg::BOX_COLS_V, Cfg::BN)) return e;
-    fp.amax = f16->amax;
-  } else {
-    if (int e = make_tmap_rows_heads(&fp.tmQ, p.q, q_rows, p.heads, DQK, p.q_row_stride, p.q_head_stride, Cfg::BOX_COLS, Cfg::BM)) return e;
-    if (int e = make_tmap_rows_heads(&fp.tmK, p.k, p.total_rows, p.heads, DQK, p.k_row_stride, p.k_head_stride, Cfg::BOX_COLS, Cfg::BN)) return e;
-    if (int e = make_tmap_rows_heads(&fp.tmV, p.v, p.total_rows, p.heads, DV, p.v_row_stride, p.v_head_stride, Cfg::BOX_COLS_V, Cfg::BN)) return e;
-  }
+  const Operands o = operands(p, f16);
+  if (int e = make_tmap_rows_heads(&fp.tmQ, o.src[0], q_rows, p.heads, DQK, o.rs[0], o.hs[0], Cfg::BOX_COLS, Cfg::BM)) return e;
+  if (int e = make_tmap_rows_heads(&fp.tmK, o.src[1], p.total_rows, p.heads, DQK, o.rs[1], o.hs[1], Cfg::BOX_COLS, Cfg::BN)) return e;
+  if (int e = make_tmap_rows_heads(&fp.tmV, o.src[2], p.total_rows, p.heads, DV, o.rs[2], o.hs[2], Cfg::BOX_COLS_V, Cfg::BN)) return e;
+  if (f16) fp.amax = f16->amax;
   fp.seq = seq_args(p);
   fp.out = p.out;
   fp.o_row_stride = p.o_row_stride;

@@ -20,9 +20,7 @@ static bool e4m3_view(const void* ptr, long long row_stride, long long head_stri
 }
 
 int e4m3_fwd_check(const hstu_attn_params& p) {
-  // dqk == dv, or dqk < dv (attn_wgmma_mixed_fwd_e4m3.cu), both in {32, 64, 128, 256}
-  auto dim_ok = [](int d) { return d == 32 || d == 64 || d == 128 || d == 256; };
-  if (p.dqk > p.dv || !dim_ok(p.dqk) || !dim_ok(p.dv)) {
+  if (!wgmma_dims(p.dqk, p.dv)) {
     set_error("fp8 attention: dqk == dv or dqk < dv, both in {32, 64, 128, 256}, only (dqk=%d, dv=%d)", p.dqk, p.dv);
     return HSTU_ERR_UNSUPPORTED;
   }
@@ -46,24 +44,14 @@ int e4m3_fwd_check(const hstu_attn_params& p) {
   return 0;
 }
 
-template <int D>
-static int launch_square(const hstu_attn_params& p, const hstu_attn_descales& ds, const void* v16, cudaStream_t st) {
-  return launch_fwd_e4m3<D, D>(p, ds, v16, st, attn_fwd_e4m3_wgmma_kernel<D>);
-}
-
 int attn_wgmma_fwd_e4m3(const hstu_attn_params& p, const hstu_attn_descales& ds, cudaStream_t st) {
   if (int e = e4m3_fwd_check(p)) return e;
   const void* v16 = nullptr;
   if (int e = e4m3_v_prepass(p, &v16, st)) return e;
   if (p.dqk != p.dv) return attn_wgmma_fwd_e4m3_mixed(p, ds, v16, st);
-  switch (p.dqk) {
-    case 32: return launch_square<32>(p, ds, v16, st);
-    case 64: return launch_square<64>(p, ds, v16, st);
-    case 128: return launch_square<128>(p, ds, v16, st);
-    case 256: return launch_square<256>(p, ds, v16, st);
-  }
-  set_error("fp8 attention: unsupported head dim %d", p.dqk);
-  return HSTU_ERR_UNSUPPORTED;
+  return dispatch_dims(SquareDims{}, p, "fp8 attention", [&]<int D, int, bool>() {
+    return launch_fwd_e4m3<D, D>(p, ds, v16, st, attn_fwd_e4m3_wgmma_kernel<D>);
+  });
 }
 
 }  // namespace hstu

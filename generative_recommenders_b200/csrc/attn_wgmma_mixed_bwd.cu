@@ -20,26 +20,11 @@ __global__ void __launch_bounds__(kAttnThreads, split_min_blocks(DV)) attn_bwd_d
   bwd_dq_body<DQK, DV, BF16>(p);
 }
 
-template <int DQK, int DV>
-static int launch_mixed(const hstu_attn_params& p, cudaStream_t st) {
-  if (p.dtype == HSTU_BF16)
-    return launch_bwd_split<DQK, DV, true>(p, st, attn_bwd_dkdv_mixed_wgmma_kernel<DQK, DV, true>,
-                                           attn_bwd_dq_mixed_wgmma_kernel<DQK, DV, true>);
-  return launch_bwd_split<DQK, DV, false>(p, st, attn_bwd_dkdv_mixed_wgmma_kernel<DQK, DV, false>,
-                                          attn_bwd_dq_mixed_wgmma_kernel<DQK, DV, false>);
-}
-
 int attn_wgmma_bwd_mixed(const hstu_attn_params& p, cudaStream_t st) {
-  switch (p.dqk * 1000 + p.dv) {
-    case 32064: return launch_mixed<32, 64>(p, st);
-    case 32128: return launch_mixed<32, 128>(p, st);
-    case 32256: return launch_mixed<32, 256>(p, st);
-    case 64128: return launch_mixed<64, 128>(p, st);
-    case 64256: return launch_mixed<64, 256>(p, st);
-    case 128256: return launch_mixed<128, 256>(p, st);
-  }
-  set_error("wgmma backward: unsupported head dims dqk = %d, dv = %d", p.dqk, p.dv);
-  return HSTU_ERR_UNSUPPORTED;
+  return dispatch_dims(MixedDims{}, p, "wgmma backward", [&]<int DQK, int DV, bool BF16>() {
+    return launch_bwd_split<DQK, DV, BF16>(p, st, attn_bwd_dkdv_mixed_wgmma_kernel<DQK, DV, BF16>,
+                                           attn_bwd_dq_mixed_wgmma_kernel<DQK, DV, BF16>);
+  });
 }
 
 }  // namespace hstu

@@ -12,22 +12,10 @@ __global__ void __launch_bounds__(kAttnThreads, kE4m3MinBlocks<DV>) attn_fwd_e4m
   attn_fwd_e4m3_body<DQK, DV>(p);
 }
 
-template <int DQK, int DV>
-static int launch_mixed(const hstu_attn_params& p, const hstu_attn_descales& ds, const void* v16, cudaStream_t st) {
-  return launch_fwd_e4m3<DQK, DV>(p, ds, v16, st, attn_fwd_e4m3_mixed_wgmma_kernel<DQK, DV>);
-}
-
 int attn_wgmma_fwd_e4m3_mixed(const hstu_attn_params& p, const hstu_attn_descales& ds, const void* v16, cudaStream_t st) {
-  switch (p.dqk * 1000 + p.dv) {
-    case 32064: return launch_mixed<32, 64>(p, ds, v16, st);
-    case 32128: return launch_mixed<32, 128>(p, ds, v16, st);
-    case 32256: return launch_mixed<32, 256>(p, ds, v16, st);
-    case 64128: return launch_mixed<64, 128>(p, ds, v16, st);
-    case 64256: return launch_mixed<64, 256>(p, ds, v16, st);
-    case 128256: return launch_mixed<128, 256>(p, ds, v16, st);
-  }
-  set_error("fp8 attention: unsupported head dims dqk = %d, dv = %d", p.dqk, p.dv);
-  return HSTU_ERR_UNSUPPORTED;
+  return dispatch_dims(MixedDims{}, p, "fp8 attention", [&]<int DQK, int DV, bool>() {
+    return launch_fwd_e4m3<DQK, DV>(p, ds, v16, st, attn_fwd_e4m3_mixed_wgmma_kernel<DQK, DV>);
+  });
 }
 
 }  // namespace hstu

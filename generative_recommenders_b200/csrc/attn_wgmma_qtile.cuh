@@ -193,4 +193,24 @@ __device__ __forceinline__ void mask_scores(const SeqMask& msk, bool fast, int f
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// host
+// ------------------------------------------------------------------------------------------------
+// SMs of an H100 SXM: the grid caps of the grid-strided helper kernels and the delta-q chunk sizing (any grid is correct)
+constexpr int kH100Sms = 132;
+
+// The q, k, v, dO views the kernels read: the inputs, or their contiguous scaled fp16 copies (f16, bf16 at d = 32)
+struct Operands {
+  const void* src[4];
+  long long rs[4], hs[4];  // row / head strides (elements)
+};
+inline Operands operands(const hstu_attn_params& p, const Fp16Operands* f16) {
+  Operands o = {{p.q, p.k, p.v, p.dout},
+                {p.q_row_stride, p.k_row_stride, p.v_row_stride, p.do_row_stride},
+                {p.q_head_stride, p.k_head_stride, p.v_head_stride, p.do_head_stride}};
+  if (f16)
+    for (int i = 0; i < 4; ++i) o.src[i] = f16->copy[i], o.rs[i] = (long long)p.heads * p.dqk, o.hs[i] = p.dqk;
+  return o;
+}
+
 }  // namespace hstu

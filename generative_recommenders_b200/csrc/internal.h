@@ -12,7 +12,44 @@ void set_error(const char* fmt, ...);
 int attn_generic_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_generic_bwd(const hstu_attn_params& p, cudaStream_t st);
 
-// attn_wgmma_fwd.cu / attn_wgmma_bwd.cu
+// The head dims of the wgmma attention kernels: dqk == dv, or dqk < dv, both in {32, 64, 128, 256}.  attn_wgmma_fwd.cu,
+// attn_wgmma_bwd.cu and attn_wgmma_fwd_e4m3.cu instantiate the square pairs, the attn_wgmma_mixed_*.cu units the others.
+template <int DQK, int DV> struct HeadDims {};
+template <class... Pairs> struct HeadDimList {};
+using SquareDims = HeadDimList<HeadDims<32, 32>, HeadDims<64, 64>, HeadDims<128, 128>, HeadDims<256, 256>>;
+using MixedDims = HeadDimList<HeadDims<32, 64>, HeadDims<32, 128>, HeadDims<32, 256>, HeadDims<64, 128>, HeadDims<64, 256>,
+                              HeadDims<128, 256>>;
+template <int... DQK, int... DV>
+constexpr bool has_dims(HeadDimList<HeadDims<DQK, DV>...>, int dqk, int dv) { return ((dqk == DQK && dv == DV) || ...); }
+inline bool wgmma_dims(int dqk, int dv) { return has_dims(SquareDims{}, dqk, dv) || has_dims(MixedDims{}, dqk, dv); }
+
+// f.template operator()<DQK, DV, BF16>() for the pair of `dims` that is (p.dqk, p.dv), with BF16 = (p.dtype == HSTU_BF16);
+// HSTU_ERR_UNSUPPORTED if there is none
+template <int... DQK, int... DV, class F>
+int dispatch_dims(HeadDimList<HeadDims<DQK, DV>...>, const hstu_attn_params& p, const char* what, F&& f) {
+  int rc = HSTU_ERR_UNSUPPORTED;
+  const bool bf = p.dtype == HSTU_BF16;
+  const bool found = ((p.dqk == DQK && p.dv == DV &&
+                       (rc = bf ? f.template operator()<DQK, DV, true>() : f.template operator()<DQK, DV, false>(), true)) || ...);
+  if (!found) set_error("%s: unsupported head dims dqk = %d, dv = %d", what, p.dqk, p.dv);
+  return rc;
+}
+
+// bf16 at dqk == dv == 32 runs the fp16 kernels on exactly scaled copies of its operands (attn_fp16_operands.cu,
+// DESIGN.md 3.0), except in the delta-q forward, which keeps the bf16 kernel.  The wgmma units instantiate no other bf16
+// kernel at these dims.
+constexpr bool scaled_fp16_dims(bool bf16, int dqk, int dv) { return bf16 && dqk == 32 && dv == 32; }
+inline bool runs_on_fp16_operands(const hstu_attn_params& p) {
+  return scaled_fp16_dims(p.dtype == HSTU_BF16, p.dqk, p.dv) && p.delta_q_len == 0;
+}
+// The fused backward kernel (dK, dV and dQ atomics into an fp32 workspace) exists at d = 64 and 128.  The backward splits
+// into atomic-free dK / dV and dQ kernels at every other dim, at dqk < dv, and when it must be deterministic (DESIGN.md
+// 3.2); at d = 256 the fused kernel's fp32 dQ accumulator would be L * H * 1 KB.
+constexpr bool fused_bwd_dims(int dqk, int dv) { return dqk == dv && (dqk == 64 || dqk == 128); }
+inline bool split_dq(const hstu_attn_params& p) { return !fused_bwd_dims(p.dqk, p.dv) || p.deterministic != 0; }
+
+// attn_wgmma_fwd.cu: whether the wgmma kernels take the call (dtype, dims, bias, views; sm_90) and the forward;
+// attn_wgmma_bwd.cu: the workspace and the backward
 bool wgmma_supported(const hstu_attn_params& p, bool bwd);
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
@@ -22,10 +59,8 @@ int attn_wgmma_bwd_on_fp16_operands(const hstu_attn_params& p, const void* kept,
 // attn_wgmma_mixed_fwd.cu / attn_wgmma_mixed_bwd.cu: the same at dqk < dv (both in {32, 64, 128, 256})
 int attn_wgmma_fwd_mixed(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd_mixed(const hstu_attn_params& p, cudaStream_t st);
-// attn_wgmma_fwd.cu: a 16-bit view the kernels take (16-byte base, row / head strides of whole 16-byte units), and whether
-// the wgmma forward takes the call (dtype, dims, alignment of q, k, v, out; sm_90)
+// attn_wgmma_fwd.cu: a 16-bit view the kernels take (16-byte base, row / head strides of whole 16-byte units)
 bool aligned_view(const void* ptr, long long row_stride, long long head_stride);
-bool wgmma_fwd_supported(const hstu_attn_params& p);
 // the delta-q forward's fp32 partials of its key chunks (0 when one chunk suffices); sizes only
 size_t wgmma_delta_workspace_bytes(const hstu_attn_params& p);
 
