@@ -72,6 +72,8 @@ _PROTOS = {
     "hstu_attn_fwd": (C.c_int, [C.POINTER(AttnParams), _vp]),
     "hstu_attn_bwd": (C.c_int, [C.POINTER(AttnParams), _vp]),
     "hstu_attn_fwd_fp8": (C.c_int, [C.POINTER(AttnParams), C.POINTER(Descales), _vp]),
+    "hstu_attn_fwd_delta_fp8_kv": (C.c_int, [C.POINTER(AttnParams), C.POINTER(Descales), _vp]),
+    "hstu_attn_fp8_kv_workspace_bytes": (C.c_size_t, [C.POINTER(AttnParams)]),
     "hstu_attn_select_impl": (C.c_int, [C.POINTER(AttnParams), C.c_int]),
     "hstu_attn_fp16_operands_bytes": (C.c_size_t, [C.POINTER(AttnParams)]),
     "hstu_attn_fwd_keep_fp16_operands": (C.c_int, [C.POINTER(AttnParams), _vp, C.c_size_t, _vp]),

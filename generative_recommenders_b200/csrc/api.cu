@@ -198,6 +198,30 @@ int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* desca
   return attn_wgmma_fwd_e4m3(*p, descales ? *descales : none, (cudaStream_t)stream);
 }
 
+int hstu_attn_fwd_delta_fp8_kv(const hstu_attn_params* p, const hstu_attn_descales* descales, void* stream) {
+  if (int e = validate_attn(p, false)) return e;
+  HSTU_CHECK_ARG(descales == nullptr || descales->q == nullptr,
+                 "hstu_attn_fwd_delta_fp8_kv: q is bf16 / fp16 and takes no descale (descales->q must be NULL)");
+  if (int e = validate_descales(descales)) return e;
+  if (int e = delta_fp8_kv_check(*p)) return e;
+  if (p->batch == 0 || p->total_rows == 0) return 0;
+  if (int e = bind_device(p->q)) return e;
+  if (int e = check_descale_devices(descales)) return e;
+  if (!is_sm90()) {
+    set_error("hstu_attn_fwd_delta_fp8_kv: the fp8 K / V kernels need an sm_90 device");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  hstu_attn_descales none;
+  memset(&none, 0, sizeof(none));
+  return attn_wgmma_fwd_delta_fp8_kv(*p, descales ? *descales : none, (cudaStream_t)stream);
+}
+
+size_t hstu_attn_fp8_kv_workspace_bytes(const hstu_attn_params* p) {
+  if (p == nullptr || validate_attn(p, false) != 0 || p->batch == 0 || p->total_rows == 0) return 0;
+  if (delta_fp8_kv_check(*p) != 0) return 0;
+  return wgmma_delta_workspace_bytes(*p);  // the partials of the key chunks, by the rule of the 16-bit delta-q forward
+}
+
 size_t hstu_attn_fp16_operands_bytes(const hstu_attn_params* p) {
   if (p == nullptr || validate_attn(p, false) != 0) return 0;
   if (p->batch == 0 || p->total_rows == 0 || !wgmma_on_fp16_operands(p, false)) return 0;

@@ -15,7 +15,7 @@ __global__ void __launch_bounds__(kAttnThreads, kE4m3MinBlocks<D>) attn_fwd_e4m3
 // host
 // ------------------------------------------------------------------------------------------------
 // fp8 views: 16-byte base, and row / head strides of whole 16-byte units (TMA strides and the pre-pass's 8-byte loads)
-static bool e4m3_view(const void* ptr, long long row_stride, long long head_stride) {
+bool e4m3_view(const void* ptr, long long row_stride, long long head_stride) {
   return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && (row_stride % 16) == 0 && (head_stride % 16) == 0;
 }
 

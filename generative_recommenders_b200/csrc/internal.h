@@ -88,7 +88,15 @@ int e4m3_fwd_check(const hstu_attn_params& p);
 int attn_wgmma_fwd_e4m3(const hstu_attn_params& p, const hstu_attn_descales& ds, cudaStream_t st);
 // attn_wgmma_mixed_fwd_e4m3.cu: its dqk < dv kernels, on the fp16 copy v16 of v that attn_wgmma_fwd_e4m3 has written
 int attn_wgmma_fwd_e4m3_mixed(const hstu_attn_params& p, const hstu_attn_descales& ds, const void* v16, cudaStream_t st);
+// attn_wgmma_fwd_e4m3.cu: an e4m3 view the kernels take (16-byte base, row / head strides of whole 16-byte units)
+bool e4m3_view(const void* ptr, long long row_stride, long long head_stride);
 bool is_sm90();
+
+// attn_wgmma_delta_fp8kv.cu: the delta-q forward with 16-bit q and out over an e4m3 K / V cache (DESIGN.md 3.8).
+// delta_fp8_kv_check: 0 if its kernels take the call (dtype, delta, bias, impl, dims, row limits, views; no device query),
+// else HSTU_ERR_UNSUPPORTED with a message
+int delta_fp8_kv_check(const hstu_attn_params& p);
+int attn_wgmma_fwd_delta_fp8_kv(const hstu_attn_params& p, const hstu_attn_descales& ds, cudaStream_t st);
 
 // norm.cu
 int layer_norm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, long long n, int D,

@@ -90,6 +90,14 @@ def cuda_hstu_attention_fwd(
     """descales: (q_descale, k_descale, v_descale) of fp8 inputs -- see cuda_hstu_attention_fwd_fp8.  q, k, v of dtype
     torch.float8_e4m3fn take that path with or without descales.  fp16_operands: an empty Fp16Operands that keeps the
     call's fp16 operands for its backward, if it runs on them."""
+    if delta_q_len and q.dtype in (torch.bfloat16, torch.float16) and k.dtype == _FP8 and v.dtype == _FP8:
+        if bias is not None:
+            raise RuntimeError("delta-q attention on an fp8 K / V cache: the relative bias is not supported")
+        if descales is not None and descales[0] is not None:
+            raise RuntimeError("delta-q attention on an fp8 K / V cache: q is bf16 / fp16 and takes no descale")
+        return cuda_hstu_attention_fwd_delta_fp8_kv(max_seq_len, alpha, q, k, v, seq_offsets, delta_q_len,
+                                                    None if descales is None else tuple(descales[1:]), num_targets,
+                                                    max_attn_len, contextual_seq_len, min_full_attn_seq_len, impl, out)
     if descales is not None or any(t.dtype == _FP8 for t in (q, k, v)):
         if bias is not None or delta_q_len:
             raise RuntimeError("fp8 attention: the relative bias and delta_q are not supported")
@@ -177,6 +185,69 @@ def cuda_hstu_attention_fwd_fp8(
     with torch.cuda.device(dev), _lib.timed("attn_fwd_fp8", dev):
         _lib.check(_lib.lib().hstu_attn_fwd_fp8(C.byref(p), C.byref(ds), _lib.stream_ptr(dev)), "hstu_attn_fwd_fp8")
     _lib.note_launch(2)  # the fp16 copy of v, then the attention kernel
+    del ws
+    return out
+
+
+def _fill_descales(ds, names, descales, B, H, dev, what):
+    for name, d in zip(names, descales):
+        if d is None:
+            continue
+        if d.dtype != torch.float32 or tuple(d.shape) != (B, H):
+            raise RuntimeError(f"{what}: {name}_descale must be an fp32 [B, H] = [{B}, {H}] tensor "
+                               f"(got {d.dtype} {tuple(d.shape)})")
+        if d.device != dev:
+            raise RuntimeError(f"{what}: {name}_descale is on {d.device}, the inputs on {dev}")
+        setattr(ds, name, d.data_ptr())
+        setattr(ds, f"{name}_batch_stride", d.stride(0))
+        setattr(ds, f"{name}_head_stride", d.stride(1))
+
+
+def cuda_hstu_attention_fwd_delta_fp8_kv(
+    max_seq_len: int, alpha: float, delta_q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, seq_offsets: torch.Tensor,
+    delta_q_len: int, kv_descales: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None,
+    num_targets: Optional[torch.Tensor] = None, max_attn_len: int = 0, contextual_seq_len: int = 0,
+    min_full_attn_seq_len: int = 0, impl: int = _lib.IMPL_AUTO, out: Optional[torch.Tensor] = None,
+) -> torch.Tensor:
+    """KV-cached (delta-q) forward with bf16 / fp16 queries over a float8_e4m3fn K / V cache (`hstu_attn_fwd_delta_fp8_kv`):
+    the attention of delta_q [B * delta_q_len, H, dqk] over k * k_descale[b, h] and v * v_descale[b, h], in the dtype of
+    delta_q.  kv_descales: (k_descale, v_descale), each an fp32 [B, H] tensor (any strides) or None for 1.  The wgmma
+    kernels widen K / V to the query dtype inside the kernel; they take dqk == dv, or dqk < dv, with both in {32, 64, 128,
+    256}, and k / v views with row / head strides that are multiples of 16 elements.  There is no generic kernel for it."""
+    what = "delta-q attention on an fp8 K / V cache"
+    if delta_q.dtype not in (torch.bfloat16, torch.float16) or k.dtype != _FP8 or v.dtype != _FP8:
+        raise RuntimeError(f"{what}: delta_q must be bf16 / fp16 and k, v torch.float8_e4m3fn "
+                           f"(got {delta_q.dtype}, {k.dtype}, {v.dtype})")
+    if delta_q_len <= 0:
+        raise RuntimeError(f"{what}: delta_q_len must be > 0 (got {delta_q_len})")
+    if impl == _lib.IMPL_GENERIC:
+        raise RuntimeError(f"{what}: runs on the wgmma kernels only (the generic kernels take no fp8 input)")
+    dev = _lib.require_cuda(delta_q, k, v, seq_offsets, num_targets)
+    delta_q, k, v = _prep(delta_q, k, v)
+    seq_offsets = seq_offsets.contiguous()
+    if num_targets is not None:
+        num_targets = num_targets.contiguous()
+    B, H = seq_offsets.numel() - 1, delta_q.shape[1]
+    ds = _lib.Descales()
+    _fill_descales(ds, "kv", kv_descales if kv_descales is not None else (None, None), B, H, dev, what)
+    if out is None:
+        out = torch.empty((delta_q.shape[0], H, v.shape[2]), dtype=delta_q.dtype, device=dev)
+    elif out.dtype != delta_q.dtype:
+        raise RuntimeError(f"{what}: out must have the dtype of delta_q ({delta_q.dtype}, got {out.dtype})")
+    p = _lib.AttnParams()
+    _fill_common(p, max_seq_len, alpha, delta_q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
+                 min_full_attn_seq_len, impl, delta_q_len)
+    p.out = out.data_ptr()
+    p.o_row_stride, p.o_head_stride = out.stride(0), out.stride(1)
+    nbytes = _lib.lib().hstu_attn_fp8_kv_workspace_bytes(C.byref(p))
+    ws = None
+    if nbytes:
+        ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+        p.workspace, p.workspace_bytes = (ws.data_ptr() + 255) // 256 * 256, nbytes
+    with torch.cuda.device(dev), _lib.timed("attn_fwd_delta_fp8_kv", dev):
+        _lib.check(_lib.lib().hstu_attn_fwd_delta_fp8_kv(C.byref(p), C.byref(ds), _lib.stream_ptr(dev)),
+                   "hstu_attn_fwd_delta_fp8_kv")
+    _lib.note_launch(2 if ws is not None else 1)  # the attention kernel, and the reduction of split key chunks
     del ws
     return out
 
@@ -359,8 +430,12 @@ def delta_hstu_mha(
     contextual_seq_len: int = 0,
     kernel: HammerKernel = HammerKernel.CUDA,
     enable_tma: bool = False,
+    kv_descales: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None,
 ) -> torch.Tensor:
-    """Drop-in for delta_hstu_mha (hstu_attention.py:131-203): the last L//B query rows of each sequence."""
+    """Drop-in for delta_hstu_mha (hstu_attention.py:131-203): the last L//B query rows of each sequence.
+
+    k and v may be a float8_e4m3fn cache under bf16 / fp16 queries (cuda_hstu_attention_fwd_delta_fp8_kv), with
+    kv_descales = (k_descale, v_descale), fp32 [B, H] tensors or None for 1."""
     L, H, D = delta_q.shape
     B = seq_offsets.size(0) - 1
     torch._assert(max_seq_len > 0, "max_seq_len must be larger than 0")
@@ -373,7 +448,8 @@ def delta_hstu_mha(
     torch._assert(v.shape[1] == H, "wrong v shape[1]")
     require_cuda_kernel(kernel, "delta_hstu_mha")
     return cuda_hstu_attention_fwd(max_seq_len, alpha, delta_q, k, v, seq_offsets, num_targets, max_attn_len,
-                                   contextual_seq_len, 0, _lib.IMPL_AUTO, delta_q_len=L // B)
+                                   contextual_seq_len, 0, _lib.IMPL_AUTO, delta_q_len=L // B,
+                                   descales=None if kv_descales is None else (None, *kv_descales))
 
 
 class _RelBiasAttentionFunction(torch.autograd.Function):

@@ -167,6 +167,17 @@ typedef struct hstu_attn_descales {
  * hstu_attn_workspace_bytes(p, 0) bytes (an fp16 copy of v, L * H * dv * 2 rounded up to 256).
  * descales may be NULL (all scales 1). */
 int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* descales, void* cuda_stream);
+/* KV-cached (delta-q) forward with 16-bit queries over an fp8 K / V cache: p->dtype (HSTU_BF16 or HSTU_F16) is the type
+ * of q and out, k and v are float8 e4m3fn, and out = delta_attention(q, k * k_descale[b, h], v * v_descale[b, h]) with
+ * every mask option of hstu_attn_fwd.  descales->q must be NULL; descales, or its k / v, may be NULL (scale 1).  wgmma
+ * kernels only (sm_90, p->impl other than HSTU_IMPL_GENERIC): delta_q_len > 0, no relative bias, dqk == dv or dqk < dv
+ * with both in {32, 64, 128, 256}; q and out 16-byte aligned with row / head strides that are multiples of 8 elements, k
+ * and v 16-byte aligned with multiples of 16.  Anything else returns HSTU_ERR_UNSUPPORTED.  When the keys are split into
+ * chunks it needs a workspace of hstu_attn_fp8_kv_workspace_bytes(p) bytes (the fp32 partials, the rule of the 16-bit
+ * delta-q forward).  hstu_attn_select_impl and hstu_attn_workspace_bytes do not describe this entry. */
+int hstu_attn_fwd_delta_fp8_kv(const hstu_attn_params* p, const hstu_attn_descales* descales, void* cuda_stream);
+/* Workspace of hstu_attn_fwd_delta_fp8_kv (sizes only, no device query): 0 with one key chunk or a call it refuses. */
+size_t hstu_attn_fp8_kv_workspace_bytes(const hstu_attn_params* p);
 /* Which implementation a call would dispatch to: returns HSTU_IMPL_GENERIC or HSTU_IMPL_UMMA (<0 on error).  A
  * deterministic backward returns HSTU_IMPL_UMMA where the wgmma backward supports the shape (it then runs its atomic-free
  * dK / dV and dQ kernels), else HSTU_IMPL_GENERIC; HSTU_ERR_UNSUPPORTED with a relative bias, or with impl forced to
