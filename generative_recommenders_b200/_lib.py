@@ -79,9 +79,16 @@ _PROTOS = {
     "hstu_attn_fwd_keep_fp16_operands": (C.c_int, [C.POINTER(AttnParams), _vp, C.c_size_t, _vp]),
     "hstu_attn_bwd_fp16_operands_workspace_bytes": (C.c_size_t, [C.POINTER(AttnParams)]),
     "hstu_attn_bwd_on_fp16_operands": (C.c_int, [C.POINTER(AttnParams), _vp, C.c_size_t, _vp]),
+    "hstu_attn_fwd_bidir": (C.c_int, [C.POINTER(AttnParams), _vp]),
+    "hstu_attn_bwd_bidir": (C.c_int, [C.POINTER(AttnParams), _vp]),
+    "hstu_attn_bidir_workspace_bytes": (C.c_size_t, [C.POINTER(AttnParams), C.c_int]),
+    "hstu_attn_bidir_select_impl": (C.c_int, [C.POINTER(AttnParams), C.c_int]),
     "hstu_mask_valid": (C.c_int, [_i32] * 7),
     "hstu_kv_range_for_q_rows": (C.c_int, [_i32] * 7 + [C.POINTER(_i32)] * 2),
     "hstu_q_range_for_kv_rows": (C.c_int, [_i32] * 7 + [C.POINTER(_i32)] * 3),
+    "hstu_mask_valid_bidir": (C.c_int, [_i32] * 7),
+    "hstu_kv_range_for_q_rows_bidir": (C.c_int, [_i32] * 7 + [C.POINTER(_i32)] * 2),
+    "hstu_q_range_for_kv_rows_bidir": (C.c_int, [_i32] * 7 + [C.POINTER(_i32)] * 3),
     "hstu_layer_norm_fwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i64, _i64, _f32, _i32, _i32, _vp]),
     "hstu_layer_norm_bwd": (C.c_int, [_vp] * 10 + [_i64, _i32, _i64, _i64, _i64, _i32, _i32, _vp]),
     "hstu_norm_bwd_partial_rows": (_i32, []),

@@ -21,7 +21,7 @@ LIB = os.path.join(HERE, "lib", "libhstu_b200.so")
 SELFTEST_LIB = os.path.join(HERE, "lib", "libhstu_b200_selftest.so")  # test infrastructure: wgmma / TMA self test
 GEN = os.path.join(OBJ, "gen")  # generated headers (wgmma_ops.cuh, scripts/gen_wgmma_ops.py)
 SELFTEST_SOURCES = ["wgmma_selftest.cu", "tmap.cu"]
-SOURCES = ["api.cu", "attn_generic.cu", "attn_wgmma_fwd.cu", "attn_wgmma_bwd.cu", "attn_wgmma_fwd_e4m3.cu", "attn_wgmma_mixed_fwd.cu", "attn_wgmma_mixed_fwd_e4m3.cu", "attn_wgmma_mixed_bwd.cu", "attn_wgmma_delta_fp8kv.cu", "attn_fp16_operands.cu", "tmap.cu", "norm.cu", "norm_fast.cu", "jagged.cu", "position.cu", "sampled_softmax.cu", "jagged_bmm.cu"]
+SOURCES = ["api.cu", "attn_generic.cu", "attn_wgmma_fwd.cu", "attn_wgmma_bwd.cu", "attn_wgmma_fwd_e4m3.cu", "attn_wgmma_mixed_fwd.cu", "attn_wgmma_mixed_fwd_e4m3.cu", "attn_wgmma_mixed_bwd.cu", "attn_wgmma_delta_fp8kv.cu", "attn_wgmma_bidir.cu", "attn_fp16_operands.cu", "tmap.cu", "norm.cu", "norm_fast.cu", "jagged.cu", "position.cu", "sampled_softmax.cu", "jagged_bmm.cu"]
 NVCC_FLAGS = [
     "-std=c++20", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xcudafe", "--diag_suppress=177",

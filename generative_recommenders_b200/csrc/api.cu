@@ -92,6 +92,35 @@ static int select_impl(const hstu_attn_params* p, bool bwd) {
   return can ? HSTU_IMPL_UMMA : HSTU_IMPL_GENERIC;
 }
 
+// The non-causal entry points (hstu_attn_fwd_bidir / hstu_attn_bwd_bidir): the routing of select_impl with the support check
+// of the non-causal wgmma kernels (attn_wgmma_bidir.cu).  The reference's KV-cached path is causal, and there is no fp8
+// backward: delta-q, a relative bias and e4m3 inputs are refused.
+static int select_impl_bidir(const hstu_attn_params* p, bool bwd) {
+  if (p->delta_q_len > 0) {
+    set_error("non-causal attention: delta_q (the KV-cached forward) is causal only");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  if (p->pos_w != nullptr || p->ts_w != nullptr) {
+    set_error("non-causal attention: the relative bias is not supported");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  if (p->dtype == HSTU_E4M3) {
+    set_error("non-causal attention: fp8 (e4m3) inputs are not supported");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  const bool can = wgmma_bidir_supported(*p, bwd);
+  if (p->impl == HSTU_IMPL_GENERIC) return HSTU_IMPL_GENERIC;
+  if (p->impl == HSTU_IMPL_UMMA) {
+    if (!can) {
+      set_error("non-causal wgmma path does not support this problem (dtype=%d dqk=%d dv=%d): it takes bf16 / fp16 at "
+                "dqk == dv in {32, 64, 128}; d = 256, dqk != dv and fp32 run on the generic kernels", p->dtype, p->dqk, p->dv);
+      return HSTU_ERR_UNSUPPORTED;
+    }
+    return HSTU_IMPL_UMMA;
+  }
+  return can ? HSTU_IMPL_UMMA : HSTU_IMPL_GENERIC;
+}
+
 // The calls that run on scaled fp16 operands (attn_fp16_operands.cu): those of runs_on_fp16_operands on the wgmma kernels
 static bool wgmma_on_fp16_operands(const hstu_attn_params* p, bool bwd) {
   return runs_on_fp16_operands(*p) && select_impl(p, bwd) == HSTU_IMPL_UMMA;
@@ -178,6 +207,37 @@ int hstu_attn_bwd(const hstu_attn_params* p, void* stream) {
   if (impl < 0) return impl;
   if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bwd(*p, (cudaStream_t)stream);
   return attn_generic_bwd(*p, (cudaStream_t)stream);
+}
+
+int hstu_attn_bidir_select_impl(const hstu_attn_params* p, int is_backward) {
+  if (int e = validate_attn(p, is_backward != 0)) return e;
+  return select_impl_bidir(p, is_backward != 0);
+}
+
+size_t hstu_attn_bidir_workspace_bytes(const hstu_attn_params* p, int is_backward) {
+  if (p == nullptr || validate_attn(p, is_backward != 0) != 0) return 0;
+  if (p->batch == 0 || p->total_rows == 0) return 0;
+  return select_impl_bidir(p, is_backward != 0) == HSTU_IMPL_UMMA ? wgmma_bidir_workspace_bytes(*p, is_backward != 0) : 0;
+}
+
+int hstu_attn_fwd_bidir(const hstu_attn_params* p, void* stream) {
+  if (int e = validate_attn(p, false)) return e;
+  const int impl = select_impl_bidir(p, false);
+  if (impl < 0) return impl;
+  if (p->batch == 0 || p->total_rows == 0) return 0;
+  if (int e = bind_device(p->q)) return e;
+  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bidir_fwd(*p, (cudaStream_t)stream);
+  return attn_generic_fwd(*p, (cudaStream_t)stream, true);
+}
+
+int hstu_attn_bwd_bidir(const hstu_attn_params* p, void* stream) {
+  if (int e = validate_attn(p, true)) return e;
+  const int impl = select_impl_bidir(p, true);
+  if (impl < 0) return impl;
+  if (p->batch == 0 || p->total_rows == 0) return 0;
+  if (int e = bind_device(p->q)) return e;
+  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bidir_bwd(*p, (cudaStream_t)stream);
+  return attn_generic_bwd(*p, (cudaStream_t)stream, true);
 }
 
 int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* descales, void* stream) {
@@ -299,6 +359,36 @@ int hstu_q_range_for_kv_rows(int32_t len, int32_t num_targets, int32_t max_attn_
   SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
   int l, h, c;
   q_range_for_kv_rows(m, n0, n1, &l, &h, &c);
+  *lo = l;
+  *hi = h;
+  *ctx_hi = c;
+  return 0;
+}
+
+int hstu_mask_valid_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
+                          int32_t contextual_seq_len, int32_t i, int32_t j) {
+  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
+  return mask_valid_bidir(m, i, j) ? 1 : 0;
+}
+
+int hstu_kv_range_for_q_rows_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
+                                   int32_t contextual_seq_len, int32_t m0, int32_t m1, int32_t* lo, int32_t* hi) {
+  HSTU_CHECK_ARG(lo && hi && m0 >= 0 && m1 > m0 && m1 <= len, "bad row range");
+  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
+  int l, h;
+  kv_range_for_q_rows_bidir(m, m0, m1, &l, &h);
+  *lo = l;
+  *hi = h;
+  return 0;
+}
+
+int hstu_q_range_for_kv_rows_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
+                                   int32_t contextual_seq_len, int32_t n0, int32_t n1, int32_t* lo, int32_t* hi,
+                                   int32_t* ctx_hi) {
+  HSTU_CHECK_ARG(lo && hi && ctx_hi && n0 >= 0 && n1 > n0 && n1 <= len, "bad row range");
+  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
+  int l, h, c;
+  q_range_for_kv_rows_bidir(m, n0, n1, &l, &h, &c);
   *lo = l;
   *hi = h;
   *ctx_hi = c;

@@ -14,9 +14,21 @@
 // as fp32 (row pitch d+1 -> conflict-free column access); each thread owns an (R x R) micro-tile of the score
 // tile and an (R x d/16) slice of the output tile.  Backward is split into a key-stationary kernel (dK, dV) and a
 // query-stationary kernel (dQ, dpos_w, dts_w) so that no atomics are needed on dQ/dK/dV (deterministic).
+// Every kernel exists for the causal mask and, with `bidir` in its name, for the non-causal one (common.cuh: ranges and
+// mask_valid_bidir; kBidir of the bodies); the non-causal kernels take no delta-q call and no relative bias.
 #include "common.cuh"
 
 namespace hstu {
+
+template <bool kBidir>
+__device__ __forceinline__ bool pair_valid(const SeqMask& m, int i, int j) {
+  return kBidir ? mask_valid_bidir(m, i, j) : mask_valid(m, i, j);
+}
+template <bool kBidir>
+__device__ __forceinline__ void key_range(const SeqMask& m, int m0, int m1, int* lo, int* hi) {
+  if (kBidir) kv_range_for_q_rows_bidir(m, m0, m1, lo, hi);
+  else kv_range_for_q_rows(m, m0, m1, lo, hi);
+}
 
 struct GenericArgs {
   hstu_attn_params p;
@@ -89,8 +101,8 @@ __device__ __forceinline__ float bias_at(const hstu_attn_params& p, int b, int i
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-template <typename T, int TILE, int DMAX>
-__global__ void __launch_bounds__(256) attn_fwd_generic_kernel(const GenericArgs args) {
+template <typename T, int TILE, int DMAX, bool kBidir>
+__device__ __forceinline__ void attn_fwd_generic_body(const GenericArgs args) {
   const hstu_attn_params& p = args.p;
   constexpr int R = TILE / 16;
   constexpr int NC = DMAX / 16;
@@ -122,7 +134,7 @@ __global__ void __launch_bounds__(256) attn_fwd_generic_kernel(const GenericArgs
     for (int c = 0; c < NC; ++c) acc[r][c] = 0.f;
 
   int lo, hi;
-  kv_range_for_q_rows(msk, g.q_pos0 + m0, g.q_pos0 + m0 + mrows, &lo, &hi);
+  key_range<kBidir>(msk, g.q_pos0 + m0, g.q_pos0 + m0 + mrows, &lo, &hi);
   const bool has_bias = p.pos_w != nullptr || p.ts_w != nullptr;
   for (int n0 = (lo / TILE) * TILE; n0 < hi; n0 += TILE) {
     const int nrows = min(TILE, g.len - n0);
@@ -155,7 +167,7 @@ __global__ void __launch_bounds__(256) attn_fwd_generic_kernel(const GenericArgs
         const int il = ty * R + r, jl = tx + 16 * c;
         const int i = g.q_pos0 + m0 + il, j = n0 + jl;
         float pval = 0.f;
-        if (il < mrows && jl < nrows && mask_valid(msk, i, j)) {
+        if (il < mrows && jl < nrows && pair_valid<kBidir>(msk, i, j)) {
           float x = s[r][c] * p.alpha;
           if (has_bias) x += bias_at(p, b, i, j);
           pval = silu_f(x);
@@ -193,11 +205,20 @@ __global__ void __launch_bounds__(256) attn_fwd_generic_kernel(const GenericArgs
   }
 }
 
+template <typename T, int TILE, int DMAX>
+__global__ void __launch_bounds__(256) attn_fwd_generic_kernel(const GenericArgs args) {
+  attn_fwd_generic_body<T, TILE, DMAX, false>(args);
+}
+template <typename T, int TILE, int DMAX>
+__global__ void __launch_bounds__(256) attn_fwd_bidir_generic_kernel(const GenericArgs args) {
+  attn_fwd_generic_body<T, TILE, DMAX, true>(args);
+}
+
 // ------------------------------------------------------------------------------------------------
 // backward, key-stationary: dK, dV
 // ------------------------------------------------------------------------------------------------
-template <typename T, int TILE, int DMAX>
-__global__ void __launch_bounds__(256) attn_bwd_kv_generic_kernel(const GenericArgs args) {
+template <typename T, int TILE, int DMAX, bool kBidir>
+__device__ __forceinline__ void attn_bwd_kv_generic_body(const GenericArgs args) {
   const hstu_attn_params& p = args.p;
   constexpr int R = TILE / 16;
   constexpr int NC = DMAX / 16;
@@ -234,7 +255,8 @@ __global__ void __launch_bounds__(256) attn_bwd_kv_generic_kernel(const GenericA
     for (int c = 0; c < NC; ++c) adk[r][c] = adv[r][c] = 0.f;
 
   int lo, hi, ctx_hi;
-  q_range_for_kv_rows(msk, n0, n0 + nrows, &lo, &hi, &ctx_hi);
+  if (kBidir) q_range_for_kv_rows_bidir(msk, n0, n0 + nrows, &lo, &hi, &ctx_hi);
+  else q_range_for_kv_rows(msk, n0, n0 + nrows, &lo, &hi, &ctx_hi);
   const bool has_bias = p.pos_w != nullptr || p.ts_w != nullptr;
   const float inv_n = 1.0f / (float)p.max_seq_len;
   // query tiles: the contextual prefix rows [0, ctx_hi) that lie before the main range, then the main range [lo, hi)
@@ -285,7 +307,7 @@ __global__ void __launch_bounds__(256) attn_bwd_kv_generic_kernel(const GenericA
           const int il = ty * R + r, jl = tx + 16 * c;
           const int i = m0 + il, j = n0 + jl;
           float pval = 0.f, ds = 0.f;
-          if (il < mrows && jl < nrows && mask_valid(msk, i, j)) {
+          if (il < mrows && jl < nrows && pair_valid<kBidir>(msk, i, j)) {
             float x = s[r][c] * p.alpha;
             if (has_bias) x += bias_at(p, b, i, j);
             const float sg = sigmoid_f(x);
@@ -337,11 +359,20 @@ __global__ void __launch_bounds__(256) attn_bwd_kv_generic_kernel(const GenericA
   }
 }
 
+template <typename T, int TILE, int DMAX>
+__global__ void __launch_bounds__(256) attn_bwd_kv_generic_kernel(const GenericArgs args) {
+  attn_bwd_kv_generic_body<T, TILE, DMAX, false>(args);
+}
+template <typename T, int TILE, int DMAX>
+__global__ void __launch_bounds__(256) attn_bwd_kv_bidir_generic_kernel(const GenericArgs args) {
+  attn_bwd_kv_generic_body<T, TILE, DMAX, true>(args);
+}
+
 // ------------------------------------------------------------------------------------------------
 // backward, query-stationary: dQ (+ dpos_w, dts_w of the research bias)
 // ------------------------------------------------------------------------------------------------
-template <typename T, int TILE, int DMAX>
-__global__ void __launch_bounds__(256) attn_bwd_q_generic_kernel(const GenericArgs args) {
+template <typename T, int TILE, int DMAX, bool kBidir>
+__device__ __forceinline__ void attn_bwd_q_generic_body(const GenericArgs args) {
   const hstu_attn_params& p = args.p;
   constexpr int R = TILE / 16;
   constexpr int NC = DMAX / 16;
@@ -379,7 +410,7 @@ __global__ void __launch_bounds__(256) attn_bwd_q_generic_kernel(const GenericAr
 #pragma unroll
     for (int c = 0; c < NC; ++c) adq[r][c] = 0.f;
   int lo, hi;
-  kv_range_for_q_rows(msk, m0, m0 + mrows, &lo, &hi);
+  key_range<kBidir>(msk, m0, m0 + mrows, &lo, &hi);
   const bool has_bias = p.pos_w != nullptr || p.ts_w != nullptr;
   const float inv_n = 1.0f / (float)p.max_seq_len;
   for (int n0 = (lo / TILE) * TILE; n0 < hi; n0 += TILE) {
@@ -425,7 +456,7 @@ __global__ void __launch_bounds__(256) attn_bwd_q_generic_kernel(const GenericAr
         const int i = m0 + il, j = n0 + jl;
         float ds = 0.f;
         int bk = -1;
-        if (il < mrows && jl < nrows && mask_valid(msk, i, j)) {
+        if (il < mrows && jl < nrows && pair_valid<kBidir>(msk, i, j)) {
           float x = s[r][c] * p.alpha;
           if (has_bias) {
             const int n = p.max_seq_len;
@@ -501,6 +532,15 @@ __global__ void __launch_bounds__(256) attn_bwd_q_generic_kernel(const GenericAr
   }
 }
 
+template <typename T, int TILE, int DMAX>
+__global__ void __launch_bounds__(256) attn_bwd_q_generic_kernel(const GenericArgs args) {
+  attn_bwd_q_generic_body<T, TILE, DMAX, false>(args);
+}
+template <typename T, int TILE, int DMAX>
+__global__ void __launch_bounds__(256) attn_bwd_q_bidir_generic_kernel(const GenericArgs args) {
+  attn_bwd_q_generic_body<T, TILE, DMAX, true>(args);
+}
+
 // ------------------------------------------------------------------------------------------------
 // host launchers
 // ------------------------------------------------------------------------------------------------
@@ -511,11 +551,11 @@ static int set_smem(K kernel, size_t bytes) {
 }
 
 template <typename T, int TILE, int DMAX>
-static int launch_fwd(const hstu_attn_params& p, cudaStream_t st) {
+static int launch_fwd(const hstu_attn_params& p, cudaStream_t st, bool bidir) {
   const int nq_max = p.delta_q_len > 0 ? p.delta_q_len : p.max_seq_len;
   dim3 grid((nq_max + TILE - 1) / TILE, p.heads, p.batch);
   size_t smem = sizeof(float) * (size_t)(2 * TILE * (p.dqk + 1) + TILE * (p.dv + 1) + TILE * (TILE + 1));
-  auto kern = attn_fwd_generic_kernel<T, TILE, DMAX>;
+  auto kern = bidir ? attn_fwd_bidir_generic_kernel<T, TILE, DMAX> : attn_fwd_generic_kernel<T, TILE, DMAX>;
   if (int e = set_smem(kern, smem)) return e;
   GenericArgs a{p};
   kern<<<grid, 256, smem, st>>>(a);
@@ -524,12 +564,12 @@ static int launch_fwd(const hstu_attn_params& p, cudaStream_t st) {
 }
 
 template <typename T, int TILE, int DMAX>
-static int launch_bwd(const hstu_attn_params& p, cudaStream_t st) {
+static int launch_bwd(const hstu_attn_params& p, cudaStream_t st, bool bidir) {
   dim3 grid((p.max_seq_len + TILE - 1) / TILE, p.heads, p.batch);
   GenericArgs a{p};
   {
     size_t smem = sizeof(float) * (size_t)(2 * TILE * (p.dqk + 1) + 2 * TILE * (p.dv + 1) + 2 * TILE * (TILE + 1));
-    auto kern = attn_bwd_kv_generic_kernel<T, TILE, DMAX>;
+    auto kern = bidir ? attn_bwd_kv_bidir_generic_kernel<T, TILE, DMAX> : attn_bwd_kv_generic_kernel<T, TILE, DMAX>;
     if (int e = set_smem(kern, smem)) return e;
     kern<<<grid, 256, smem, st>>>(a);
     HSTU_CUDA_OK(cudaGetLastError());
@@ -537,7 +577,7 @@ static int launch_bwd(const hstu_attn_params& p, cudaStream_t st) {
   {
     size_t smem = sizeof(float) * (size_t)(2 * TILE * (p.dqk + 1) + 2 * TILE * (p.dv + 1) + TILE * (TILE + 1) + 2 * TILE +
                                            (p.dts_w ? p.num_ts_buckets + 1 : 0));
-    auto kern = attn_bwd_q_generic_kernel<T, TILE, DMAX>;
+    auto kern = bidir ? attn_bwd_q_bidir_generic_kernel<T, TILE, DMAX> : attn_bwd_q_generic_kernel<T, TILE, DMAX>;
     if (int e = set_smem(kern, smem)) return e;
     kern<<<grid, 256, smem, st>>>(a);
     HSTU_CUDA_OK(cudaGetLastError());
@@ -546,35 +586,35 @@ static int launch_bwd(const hstu_attn_params& p, cudaStream_t st) {
 }
 
 template <typename T>
-static int dispatch_fwd(const hstu_attn_params& p, cudaStream_t st) {
+static int dispatch_fwd(const hstu_attn_params& p, cudaStream_t st, bool bidir) {
   const int dm = p.dqk > p.dv ? p.dqk : p.dv;
-  if (dm <= 64) return launch_fwd<T, 64, 64>(p, st);
-  if (dm <= 128) return launch_fwd<T, 64, 128>(p, st);
-  return launch_fwd<T, 64, 256>(p, st);
+  if (dm <= 64) return launch_fwd<T, 64, 64>(p, st, bidir);
+  if (dm <= 128) return launch_fwd<T, 64, 128>(p, st, bidir);
+  return launch_fwd<T, 64, 256>(p, st, bidir);
 }
 template <typename T>
-static int dispatch_bwd(const hstu_attn_params& p, cudaStream_t st) {
+static int dispatch_bwd(const hstu_attn_params& p, cudaStream_t st, bool bidir) {
   const int dm = p.dqk > p.dv ? p.dqk : p.dv;
-  if (dm <= 64) return launch_bwd<T, 64, 64>(p, st);
-  if (dm <= 128) return launch_bwd<T, 64, 128>(p, st);
-  return launch_bwd<T, 32, 256>(p, st);
+  if (dm <= 64) return launch_bwd<T, 64, 64>(p, st, bidir);
+  if (dm <= 128) return launch_bwd<T, 64, 128>(p, st, bidir);
+  return launch_bwd<T, 32, 256>(p, st, bidir);
 }
 
-int attn_generic_fwd(const hstu_attn_params& p, cudaStream_t st) {
+int attn_generic_fwd(const hstu_attn_params& p, cudaStream_t st, bool bidir) {
   switch (p.dtype) {
-    case HSTU_F32: return dispatch_fwd<float>(p, st);
-    case HSTU_BF16: return dispatch_fwd<__nv_bfloat16>(p, st);
-    case HSTU_F16: return dispatch_fwd<__half>(p, st);
+    case HSTU_F32: return dispatch_fwd<float>(p, st, bidir);
+    case HSTU_BF16: return dispatch_fwd<__nv_bfloat16>(p, st, bidir);
+    case HSTU_F16: return dispatch_fwd<__half>(p, st, bidir);
   }
   set_error("unsupported dtype %d", p.dtype);
   return HSTU_ERR_UNSUPPORTED;
 }
 
-int attn_generic_bwd(const hstu_attn_params& p, cudaStream_t st) {
+int attn_generic_bwd(const hstu_attn_params& p, cudaStream_t st, bool bidir) {
   switch (p.dtype) {
-    case HSTU_F32: return dispatch_bwd<float>(p, st);
-    case HSTU_BF16: return dispatch_bwd<__nv_bfloat16>(p, st);
-    case HSTU_F16: return dispatch_bwd<__half>(p, st);
+    case HSTU_F32: return dispatch_bwd<float>(p, st, bidir);
+    case HSTU_BF16: return dispatch_bwd<__nv_bfloat16>(p, st, bidir);
+    case HSTU_F16: return dispatch_bwd<__half>(p, st, bidir);
   }
   set_error("unsupported dtype %d", p.dtype);
   return HSTU_ERR_UNSUPPORTED;

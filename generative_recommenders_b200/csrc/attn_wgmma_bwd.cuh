@@ -153,8 +153,11 @@ struct QTiles {
 // sequence end).  With Cfg::NSL > 1 slices, NSL CTAs share a key tile: CTA x takes key tile x / NSL, dK columns
 // [ck0, ck0 + DQK / NSL) and dV columns [cv0, cv0 + DV / NSL), ck0 = DQK / NSL (x % NSL) and cv0 likewise; its S^T / dP^T MMAs
 // still reduce over all DQK / DV columns.
-template <int DQK, int DV, bool BF16, bool FUSED_DQ>
+// kBidir: the non-causal mask (attn_wgmma_bidir.cu; split kernels only): the query range of q_range_for_kv_rows_bidir and
+// its mask cases, nothing else.
+template <int DQK, int DV, bool BF16, bool FUSED_DQ, bool kBidir = false>
 __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
+  static_assert(!(FUSED_DQ && kBidir), "the non-causal backward runs the split kernels");
   using Cfg = BwdCfg<DQK, DV, FUSED_DQ>;
   constexpr int SW = Cfg::SW, SWQ = Cfg::SWQ, SWV = Cfg::SWV, BQ = Cfg::BQ, NST = Cfg::STAGES;
   constexpr int NSL = Cfg::NSL, DNK = DQK / NSL, DNV = DV / NSL;  // column slices per key tile, and their widths
@@ -178,7 +181,8 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
   QTiles qt;
   {
     int lo, hi, ctx_hi;
-    q_range_for_kv_rows(msk, n0, n0 + nrows, &lo, &hi, &ctx_hi);
+    if constexpr (kBidir) q_range_for_kv_rows_bidir(msk, n0, n0 + nrows, &lo, &hi, &ctx_hi);
+    else q_range_for_kv_rows(msk, n0, n0 + nrows, &lo, &hi, &ctx_hi);
     qt.A = (ctx_hi + BQ - 1) / BQ;
     qt.first = max(lo / BQ, qt.A);
     qt.T = qt.A + max(0, (hi + BQ - 1) / BQ - qt.first);
@@ -302,7 +306,30 @@ __device__ __forceinline__ void bwd_key_tile(const BwdParams& p) {
       s[n] = v ? pv : 0.f;
       dp[n] = v ? dsv : 0.f;
     };
-    if (fast && keys_hist && n0 + Cfg::BKV <= q0 && q0 + BQ <= len) {  // tile-uniform: every pair valid
+    if constexpr (kBidir) {
+      // the cases of mask_scores_bidir (attn_wgmma_qtile.cuh), here with the key rows fixed and the query tile streamed
+      if (n0 + Cfg::BKV <= len && q0 + BQ <= len && bidir_block_all_valid(msk, q0, q0 + BQ, n0, n0 + Cfg::BKV)) {
+#pragma unroll
+        for (int n = 0; n < BQ / 2; ++n) score(n, true);
+      } else if (msk.win == 0 && msk.max_id >= 1) {
+        const int t_first = target_start(msk);
+#pragma unroll
+        for (int nb = 0; nb < BQ / 8; ++nb)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int kj = k_base + (e >> 1) * 8, qi = q0 + nb * 8 + 2 * t4 + (e & 1);
+            score(nb * 4 + e, kj < len && qi < len && (qi < t_first || kj < t_first || kj == qi));
+          }
+      } else {
+#pragma unroll
+        for (int nb = 0; nb < BQ / 8; ++nb)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int kj = k_base + (e >> 1) * 8, qi = q0 + nb * 8 + 2 * t4 + (e & 1);
+            score(nb * 4 + e, kj < len && qi < len && mask_valid_bidir(msk, qi, kj));
+          }
+      }
+    } else if (fast && keys_hist && n0 + Cfg::BKV <= q0 && q0 + BQ <= len) {  // tile-uniform: every pair valid
 #pragma unroll
       for (int n = 0; n < BQ / 2; ++n) score(n, true);
     } else if (fast) {
@@ -493,7 +520,8 @@ struct DqCfg {
 // Per 64-key tile each warpgroup runs S = Q K^T and dP = dO V^T (A and B K-major), releases V, forms
 // 2 dS N / alpha = dP (1 + g2) * mask from one tanh, and runs dQ += dS K (A from registers, K read MN-major), then releases K.
 // Q, K and dQ are DQK wide, dO and V DV wide.
-template <int DQK, int DV, bool BF16>
+// kBidir: the non-causal mask (attn_wgmma_bidir.cu): the key range and mask cases of the non-causal forward, nothing else.
+template <int DQK, int DV, bool BF16, bool kBidir = false>
 __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
   using Cfg = DqCfg<DQK, DV>;
   constexpr int SW = Cfg::SW, SWV = Cfg::SWV, BN = Cfg::BN, NST = Cfg::STAGES;
@@ -501,7 +529,7 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
   const int b = blockIdx.z, h = blockIdx.y;
   const int m0 = (int)(gridDim.x - 1 - blockIdx.x) * Cfg::BM;
   QTileSeq qs;  // (rows past max_seq_len get zero gradients)
-  if (!qtile_prologue<Cfg::BM, BN>(p.seq, b, h, m0, p.dq, p.dq_row_stride, p.dq_head_stride, DQK, &qs)) return;
+  if (!qtile_prologue<Cfg::BM, BN, kBidir>(p.seq, b, h, m0, p.dq, p.dq_row_stride, p.dq_head_stride, DQK, &qs)) return;
 
   uint8_t* smem = dyn_smem_1k();
   // V of tile i is released once the warp's S / dP MMAs have completed, K once its dQ MMAs have
@@ -589,7 +617,8 @@ __device__ __forceinline__ void bwd_dq_body(const BwdParams& p) {
       if (kScaled) dsv *= sc.c_d;
       return dsv;
     };
-    mask_scores<BN>(qs.msk, fast, full_lim, qs.len, q_base, n0, t4, dp, dscore);
+    if constexpr (kBidir) mask_scores_bidir<BN>(qs.msk, qs.len, m0, m0 + qs.mrows, q_base, n0, t4, dp, dscore);
+    else mask_scores<BN>(qs.msk, fast, full_lim, qs.len, q_base, n0, t4, dp, dscore);
 #pragma unroll
     for (int kk = 0; kk < BN / 16; ++kk) {
 #pragma unroll

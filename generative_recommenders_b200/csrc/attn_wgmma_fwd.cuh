@@ -101,10 +101,12 @@ __device__ __forceinline__ DeltaRows delta_rows(const FwdParams& p) {
 }
 
 // kDelta: the delta-q geometry and key chunks described at the top (grid (B * H, query tiles, chunks)); otherwise the full
-// attention of grid (query tiles, H, B).  Its only instantiations are the kernels of attn_wgmma_fwd.cu and
-// attn_wgmma_mixed_fwd.cu.
-template <int DQK, int DV, bool BF16, bool kDelta>
+// attention of grid (query tiles, H, B).  kBidir: the non-causal mask (attn_wgmma_bidir.cu; full attention only): the key
+// range of kv_range_for_q_rows_bidir and the mask cases of mask_scores_bidir, nothing else.  Its only instantiations are
+// the kernels of attn_wgmma_fwd.cu, attn_wgmma_mixed_fwd.cu and attn_wgmma_bidir.cu.
+template <int DQK, int DV, bool BF16, bool kDelta, bool kBidir = false>
 __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
+  static_assert(!(kDelta && kBidir), "the delta-q forward is causal");
   using Cfg = FwdCfg<DQK, DV>;
   constexpr int SW = Cfg::SW, SWV = Cfg::SWV, BN = Cfg::BN, NST = Cfg::STAGES;
   // dv <= 64: P V of tile i and S of tile i + 1 form one MMA batch with one wait (both fit in 128 registers); larger dv waits
@@ -119,7 +121,7 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
     return;
   }
   const int p0 = kDelta ? qs.len - p.delta + m0 : m0;  // sequence position of query row m0 (delta: the last delta rows)
-  key_tiles<Cfg::BM, BN>(p.seq, b, p0, (kDelta ? p.delta : qs.len) - m0, &qs);
+  key_tiles<Cfg::BM, BN, kBidir>(p.seq, b, p0, (kDelta ? p.delta : qs.len) - m0, &qs);
   if constexpr (kDelta) {
     // chunk blockIdx.z of gridDim.z even shares of whole tiles; an empty share (or no key at all) writes zeros, so that
     // every partial the reduction reads is defined
@@ -243,7 +245,8 @@ __device__ __forceinline__ void attn_fwd_wgmma_body(const FwdParams& p) {
     };
     // a warp of padding rows only (delta) skips this stage: its A fragments keep the zeros they start with, so its P is 0
     if (!rows_idle) {
-      mask_scores<BN>(qs.msk, fast, full_lim, qs.len, q_base, n0, t4, s, silu);
+      if constexpr (kBidir) mask_scores_bidir<BN>(qs.msk, qs.len, p0, p0 + qs.mrows, q_base, n0, t4, s, silu);
+      else mask_scores<BN>(qs.msk, fast, full_lim, qs.len, q_base, n0, t4, s, silu);
 #pragma unroll
       for (int kk = 0; kk < BN / 16; ++kk) {
         const Operand<BF16> x0(s[8 * kk + 0], s[8 * kk + 1]), x1(s[8 * kk + 2], s[8 * kk + 3]);

@@ -57,23 +57,24 @@ __device__ __forceinline__ bool qtile_rows(const SeqArgs& a, int b, int h, int m
 }
 
 // The CTA's valid query rows, of the `rows` left from its first row on, which is at sequence position p0; the mask, and
-// the key tiles those rows attend
-template <int BM, int BN>
+// the key tiles those rows attend (kBidir: under the non-causal mask, common.cuh)
+template <int BM, int BN, bool kBidir = false>
 __device__ __forceinline__ void key_tiles(const SeqArgs& a, int b, int p0, int rows, QTileSeq* q) {
   const int n_tgt = a.num_targets ? (int)load_index(a.num_targets, a.targets_i64, b) : -1;
   q->msk = make_seq_mask(q->len, n_tgt, a.win, a.min_full, a.ctx);
   q->mrows = min(BM, rows);
   int lo, hi;
-  kv_range_for_q_rows(q->msk, p0, p0 + q->mrows, &lo, &hi);
+  if constexpr (kBidir) kv_range_for_q_rows_bidir(q->msk, p0, p0 + q->mrows, &lo, &hi);
+  else kv_range_for_q_rows(q->msk, p0, p0 + q->mrows, &lo, &hi);
   q->t0 = lo / BN;
   q->T = (hi + BN - 1) / BN - q->t0;
 }
 // Both, for a CTA whose rows [m0, m0 + BM) sit at their own positions
-template <int BM, int BN>
+template <int BM, int BN, bool kBidir = false>
 __device__ __forceinline__ bool qtile_prologue(const SeqArgs& a, int b, int h, int m0, void* out, long long row_stride,
                                                long long head_stride, int d, QTileSeq* q) {
   if (!qtile_rows(a, b, h, m0, out, row_stride, head_stride, d, q)) return false;
-  key_tiles<BM, BN>(a, b, m0, q->len - m0, q);
+  key_tiles<BM, BN, kBidir>(a, b, m0, q->len - m0, q);
   return true;
 }
 
@@ -189,6 +190,41 @@ __device__ __forceinline__ void mask_scores(const SeqMask& msk, bool fast, int f
         const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
         const float v = f(nb * 4 + e);
         x[nb * 4 + e] = (kj < len && mask_valid(msk, qi, kj)) ? v : 0.f;
+      }
+  }
+}
+
+// The same under the non-causal mask, for the CTA's query rows [q_lo, q_hi).  Cases, chosen once per tile: every pair valid
+// (bidir_block_all_valid: no target x target pair, and with a window every id distance within it) / no window: only the
+// target x target pairs off the diagonal are masked (keys and rows below t_first = target_start are never) / the general
+// mask (window edges, degenerate sequences).
+template <int BN, class F>
+__device__ __forceinline__ void mask_scores_bidir(const SeqMask& msk, int len, int q_lo, int q_hi, int q_base, int n0, int t4,
+                                                  float (&x)[BN / 2], F f) {
+  if (n0 + BN <= len && bidir_block_all_valid(msk, q_lo, q_hi, n0, n0 + BN)) {
+#pragma unroll
+    for (int n = 0; n < BN / 2; ++n) x[n] = f(n);
+  } else if (msk.win == 0 && msk.max_id >= 1) {
+    const int t_first = target_start(msk);
+    bool row_hist[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) row_hist[hh] = q_base + hh * 8 < t_first;
+#pragma unroll
+    for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+        const float v = f(nb * 4 + e);
+        x[nb * 4 + e] = (kj < len && (row_hist[e >> 1] || kj < t_first || kj == qi)) ? v : 0.f;
+      }
+  } else {
+#pragma unroll
+    for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int qi = q_base + (e >> 1) * 8, kj = n0 + nb * 8 + 2 * t4 + (e & 1);
+        const float v = f(nb * 4 + e);
+        x[nb * 4 + e] = (kj < len && mask_valid_bidir(msk, qi, kj)) ? v : 0.f;
       }
   }
 }

@@ -156,6 +156,95 @@ __host__ __device__ inline void q_range_for_kv_rows(const SeqMask& m, int n0, in
 }
 
 // ------------------------------------------------------------------------------------------------
+// Non-causal (bidirectional) mask: _get_valid_attn_mask(causal=False) of pt_hstu_attention.py:33-84.  The ids are those of
+// the causal mask; dist = |id_i - id_j|; valid = (i == j) | (dist > 0), then max_attn_len / min_full_attn_seq_len on dist,
+// then the contextual rule.  So history rows see the target keys, and a target row sees every history key (within the
+// window) but of the target keys only its own.  SeqMask::fast is not used here.
+// ------------------------------------------------------------------------------------------------
+__host__ __device__ inline bool mask_valid_bidir(const SeqMask& m, int i, int j) {
+  const int idi = seq_id(m, i), idj = seq_id(m, j);
+  const int d = idi > idj ? idi - idj : idj - idi;
+  bool valid = (i == j) | (d > 0);
+  if (m.win > 0) {
+    if (m.min_full > 0)
+      valid = valid & ((d <= m.win) | (idi >= m.max_id - m.min_full));
+    else
+      valid = valid & (d <= m.win);
+  }
+  if (m.ctx > 0) valid = valid | ((idi == 0) & (idj < m.max_id));
+  return valid;
+}
+
+// First position of the target block (id == max_id); len without targets
+__host__ __device__ inline int target_start(const SeqMask& m) {
+  if (!m.has_tgt) return m.len;
+  if (m.max_id <= 0) return 0;
+  const int t = m.max_id + (m.ctx > 0 ? m.ctx - 1 : 0);
+  return t < m.len ? t : m.len;
+}
+
+// Positions [lo, hi) whose id lies in [a, b] (ids do not decrease along the sequence); a <= max_id
+__host__ __device__ inline void positions_of_ids(const SeqMask& m, int a, int b, int* lo, int* hi) {
+  const long long off = m.ctx > 0 ? m.ctx - 1 : 0;
+  long long l = a <= 0 ? 0 : a + off;
+  long long h = (m.has_tgt && b >= m.max_id) ? m.len : (long long)b + off + 1;
+  *lo = (int)(l < m.len ? l : m.len);
+  *hi = (int)(h < 0 ? 0 : h < m.len ? h : m.len);
+}
+
+// Key range [lo, hi) attended by query rows [m0, m1) (m1 <= len).  [0, len) without a window (exact); with one, the keys
+// within max_attn_len of the rows' ids and the diagonal, widened to [0, len) for rows of the full-attention tail
+// (min_full_attn_seq_len) and for contextual rows.
+__host__ __device__ inline void kv_range_for_q_rows_bidir(const SeqMask& m, int m0, int m1, int* lo, int* hi) {
+  int l = 0, h = m.len;
+  if (m.win > 0 && m.max_id >= 1) {
+    const bool full_rows = (m.min_full > 0 && seq_id(m, m1 - 1) >= m.max_id - m.min_full) || (m.ctx > 0 && m0 < m.ctx);
+    if (!full_rows) {
+      positions_of_ids(m, seq_id(m, m0) - m.win, seq_id(m, m1 - 1) + m.win, &l, &h);
+      if (l > m0) l = m0;
+      if (h < m1) h = m1;
+    }
+  }
+  *lo = l;
+  *hi = h;
+}
+
+// Query range [lo, hi) attending keys [n0, n1) (n1 <= len), plus the contextual prefix rows [0, ctx_hi) before lo.
+// [0, len) without a window (exact); with one, the rows within max_attn_len of the keys' ids and the diagonal, widened to
+// the end of the sequence over the full-attention tail (min_full_attn_seq_len), plus the contextual rows.
+__host__ __device__ inline void q_range_for_kv_rows_bidir(const SeqMask& m, int n0, int n1, int* lo, int* hi, int* ctx_hi) {
+  int l = 0, h = m.len, c = 0;
+  if (m.win > 0 && m.max_id >= 1) {
+    positions_of_ids(m, seq_id(m, n0) - m.win, seq_id(m, n1 - 1) + m.win, &l, &h);
+    if (l > n0) l = n0;
+    if (h < n1) h = n1;
+    if (m.min_full > 0) {  // the full-attention rows (id >= max_id - min_full) are the last ones of the sequence
+      int f, unused;
+      positions_of_ids(m, m.max_id - m.min_full, m.max_id, &f, &unused);
+      if (l > f) l = f;
+      h = m.len;
+    }
+    if (m.ctx > 0) c = m.ctx < l ? m.ctx : l;
+  }
+  *lo = l;
+  *hi = h;
+  *ctx_hi = c;
+}
+
+// Whether every pair of query rows [q0, q1) and keys [k0, k1) (both within the sequence) is valid under the bidirectional
+// mask.  Equal ids off the diagonal occur only among contextual rows (valid through the contextual rule) and among targets
+// (invalid); the window then bounds the largest id distance of the block.
+__host__ __device__ inline bool bidir_block_all_valid(const SeqMask& m, int q0, int q1, int k0, int k1) {
+  if (m.max_id < 1) return false;
+  const int t0 = target_start(m);
+  if (q1 > t0 && k1 > t0) return false;  // target x target
+  if (m.win == 0) return true;
+  if (m.min_full > 0 && seq_id(m, q0) >= m.max_id - m.min_full) return true;
+  const int a = seq_id(m, q1 - 1) - seq_id(m, k0), b = seq_id(m, k1 - 1) - seq_id(m, q0);
+  return (a > b ? a : b) <= m.win;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Per-sequence geometry read from device arrays
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ long long load_index(const void* p, int is_i64, int idx) {

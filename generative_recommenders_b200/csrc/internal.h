@@ -8,9 +8,9 @@
 namespace hstu {
 void set_error(const char* fmt, ...);
 
-// attn_generic.cu
-int attn_generic_fwd(const hstu_attn_params& p, cudaStream_t st);
-int attn_generic_bwd(const hstu_attn_params& p, cudaStream_t st);
+// attn_generic.cu (bidir: the non-causal mask of common.cuh)
+int attn_generic_fwd(const hstu_attn_params& p, cudaStream_t st, bool bidir = false);
+int attn_generic_bwd(const hstu_attn_params& p, cudaStream_t st, bool bidir = false);
 
 // The head dims of the wgmma attention kernels: dqk == dv, or dqk < dv, both in {32, 64, 128, 256}.  attn_wgmma_fwd.cu,
 // attn_wgmma_bwd.cu and attn_wgmma_fwd_e4m3.cu instantiate the square pairs, the attn_wgmma_mixed_*.cu units the others.
@@ -54,6 +54,12 @@ bool wgmma_supported(const hstu_attn_params& p, bool bwd);
 size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
+// attn_wgmma_bidir.cu: the non-causal mask at dqk == dv in {32, 64, 128}, no delta-q; wgmma_supported otherwise.  Its
+// workspace (the scaled fp16 operands of bf16 at d = 32, or 0), its forward and its (split) backward
+bool wgmma_bidir_supported(const hstu_attn_params& p, bool bwd);
+size_t wgmma_bidir_workspace_bytes(const hstu_attn_params& p, bool bwd);
+int attn_wgmma_bidir_fwd(const hstu_attn_params& p, cudaStream_t st);
+int attn_wgmma_bidir_bwd(const hstu_attn_params& p, cudaStream_t st);
 // attn_wgmma_bwd.cu: the bf16 d = 32 backward on the fp16 operands a forward kept (hstu_attn_bwd_on_fp16_operands)
 int attn_wgmma_bwd_on_fp16_operands(const hstu_attn_params& p, const void* kept, cudaStream_t st);
 // attn_wgmma_mixed_fwd.cu / attn_wgmma_mixed_bwd.cu: the same at dqk < dv (both in {32, 64, 128, 256})

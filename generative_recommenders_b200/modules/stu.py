@@ -140,6 +140,9 @@ class STULayer(STU):
 
     def cached_forward(self, delta_x, num_targets, max_kv_caching_len: int = 0,
                        kv_caching_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        if not self._causal:
+            raise RuntimeError("STULayer.cached_forward: KV-cached (delta-q) attention is causal only; this layer has "
+                               "causal=False")
         with record_function("## stu_compute_uqvk ##"):
             delta_u, delta_q, delta_k, delta_v = hstu_compute_uqvk(
                 x=delta_x, norm_weight=self._input_norm_weight.to(delta_x.dtype),

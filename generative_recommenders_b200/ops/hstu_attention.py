@@ -5,6 +5,8 @@ Same call surface as the reference facade generative_recommenders/ops/hstu_atten
 `cuda_hstu_attention_fwd/bwd` are the raw (non-autograd) entry points used by the fused block op; their
 dq/dk/dv are caller-allocated and may be strided views of one `duvqk` buffer, as in the reference's
 ops/cpp/cuda_hstu_preprocess_and_attention.py:254-306.
+`causal=False` runs the non-causal attention (`hstu_attn_fwd_bidir` / `hstu_attn_bwd_bidir`) under the reference eager
+path's causal=False mask; it takes no delta-q, fp8 input, relative bias or kept fp16 operands.
 """
 import ctypes as C
 from typing import Optional, Tuple
@@ -45,8 +47,9 @@ def _fill_common(p, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_a
     p.v_row_stride, p.v_head_stride = v.stride(0), v.stride(1)
 
 
-def _workspace(p, bwd: bool, device):
-    nbytes = _lib.lib().hstu_attn_workspace_bytes(C.byref(p), int(bwd))
+def _workspace(p, bwd: bool, device, causal: bool = True):
+    size = _lib.lib().hstu_attn_workspace_bytes if causal else _lib.lib().hstu_attn_bidir_workspace_bytes
+    nbytes = size(C.byref(p), int(bwd))
     if nbytes == 0:
         p.workspace, p.workspace_bytes = None, 0
         return None
@@ -85,12 +88,16 @@ def cuda_hstu_attention_fwd(
     min_full_attn_seq_len: int = 0, impl: int = _lib.IMPL_AUTO, delta_q_len: int = 0,
     out: Optional[torch.Tensor] = None, bias: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
     descales: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor], Optional[torch.Tensor]]] = None,
-    fp16_operands: Optional[Fp16Operands] = None,
+    fp16_operands: Optional[Fp16Operands] = None, causal: bool = True,
 ) -> torch.Tensor:
     """descales: (q_descale, k_descale, v_descale) of fp8 inputs -- see cuda_hstu_attention_fwd_fp8.  q, k, v of dtype
     torch.float8_e4m3fn take that path with or without descales.  fp16_operands: an empty Fp16Operands that keeps the
-    call's fp16 operands for its backward, if it runs on them."""
-    if delta_q_len and q.dtype in (torch.bfloat16, torch.float16) and k.dtype == _FP8 and v.dtype == _FP8:
+    call's fp16 operands for its backward, if it runs on them (a non-causal call leaves it empty).  causal=False: the
+    non-causal attention (bf16 / fp16 / fp32, no delta_q, fp8 or bias)."""
+    if not causal:
+        _refuse_bidir(q, k, v, delta_q_len, bias, descales)
+        fp16_operands = None
+    elif delta_q_len and q.dtype in (torch.bfloat16, torch.float16) and k.dtype == _FP8 and v.dtype == _FP8:
         if bias is not None:
             raise RuntimeError("delta-q attention on an fp8 K / V cache: the relative bias is not supported")
         if descales is not None and descales[0] is not None:
@@ -98,7 +105,7 @@ def cuda_hstu_attention_fwd(
         return cuda_hstu_attention_fwd_delta_fp8_kv(max_seq_len, alpha, q, k, v, seq_offsets, delta_q_len,
                                                     None if descales is None else tuple(descales[1:]), num_targets,
                                                     max_attn_len, contextual_seq_len, min_full_attn_seq_len, impl, out)
-    if descales is not None or any(t.dtype == _FP8 for t in (q, k, v)):
+    elif descales is not None or any(t.dtype == _FP8 for t in (q, k, v)):
         if bias is not None or delta_q_len:
             raise RuntimeError("fp8 attention: the relative bias and delta_q are not supported")
         return cuda_hstu_attention_fwd_fp8(max_seq_len, alpha, q, k, v, seq_offsets, descales, num_targets, max_attn_len,
@@ -126,9 +133,10 @@ def cuda_hstu_attention_fwd(
             _lib.check(_lib.lib().hstu_attn_fwd_keep_fp16_operands(C.byref(p), fp16_operands.base, kept, _lib.stream_ptr(dev)),
                        "hstu_attn_fwd_keep_fp16_operands")
     else:
-        ws = _workspace(p, False, dev)
-        with torch.cuda.device(dev), _lib.timed("attn_fwd", dev):
-            _lib.check(_lib.lib().hstu_attn_fwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_fwd")
+        ws = _workspace(p, False, dev) if causal else _workspace(p, False, dev, causal=False)
+        name = "hstu_attn_fwd" if causal else "hstu_attn_fwd_bidir"
+        with torch.cuda.device(dev), _lib.timed(name[len("hstu_"):], dev):
+            _lib.check(getattr(_lib.lib(), name)(C.byref(p), _lib.stream_ptr(dev)), name)
     if delta_q_len:  # a workspace holds the partials of split key chunks: the attention kernel, then their reduction
         _lib.note_launch(2 if ws is not None else 1)
     else:  # bf16 at d = 32: amax and convert kernels before the attention kernel (into the workspace or the operands buffer)
@@ -138,6 +146,15 @@ def cuda_hstu_attention_fwd(
 
 
 _FP8 = torch.float8_e4m3fn
+
+
+def _refuse_bidir(q, k, v, delta_q_len=0, bias=None, descales=None):
+    if delta_q_len:
+        raise RuntimeError("non-causal attention: delta_q (the KV-cached forward) is causal only")
+    if descales is not None or any(t is not None and t.dtype == _FP8 for t in (q, k, v)):
+        raise RuntimeError("non-causal attention: fp8 (float8_e4m3fn) inputs are not supported")
+    if bias is not None:
+        raise RuntimeError("non-causal attention: the relative bias is not supported")
 
 
 def cuda_hstu_attention_fwd_fp8(
@@ -260,9 +277,12 @@ def cuda_hstu_attention_bwd(
     bias: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None,
     dbias: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
     deterministic: Optional[bool] = None,
-    fp16_operands: Optional[Fp16Operands] = None,
+    fp16_operands: Optional[Fp16Operands] = None, causal: bool = True,
 ) -> None:
     """Writes dq, dk, dv in place (last-dim stride 1 required; row/head strides arbitrary).
+
+    causal=False: the backward of the non-causal attention.  It runs atomic-free kernels on every path, so it is bitwise
+    reproducible whatever `deterministic` says; it takes no relative bias and no kept fp16 operands.
 
     fp16_operands: what the forward of these q, k, v kept (Fp16Operands).  If it holds operands, q, k, v are not read and may
     be None; that backward runs on the wgmma kernels only, so a dout or dq / dk / dv view they cannot take goes through a
@@ -275,6 +295,10 @@ def cuda_hstu_attention_bwd(
     if deterministic is None:
         deterministic = torch.are_deterministic_algorithms_enabled()
     kept = fp16_operands is not None and fp16_operands.buf is not None
+    if not causal:
+        if kept:
+            raise RuntimeError("non-causal attention: a non-causal forward keeps no fp16 operands; pass q, k, v")
+        _refuse_bidir(q, k, v, bias=bias)
     if kept and q is None:  # dqk == dv: dout has the shape and dtype of q, k and v
         q = k = v = dout
     dev = _lib.require_cuda(dout, q, k, v, dq, dk, dv, seq_offsets, num_targets)
@@ -313,11 +337,13 @@ def cuda_hstu_attention_bwd(
                 g.copy_(w)
         del ws, keep
         return
-    ws = _workspace(p, True, dev)
-    with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
-        _lib.check(_lib.lib().hstu_attn_bwd(C.byref(p), _lib.stream_ptr(dev)), "hstu_attn_bwd")
-    # wgmma path: dK/dV kernel + dQ kernel (d = 32, after the amax and convert kernels for bf16; deterministic d = 64 / 128:
-    # no workspace, no memset, no convert) or main kernel + dQ convert; generic path: dK/dV kernel + dQ kernel
+    ws = _workspace(p, True, dev) if causal else _workspace(p, True, dev, causal=False)
+    name = "hstu_attn_bwd" if causal else "hstu_attn_bwd_bidir"
+    with torch.cuda.device(dev), _lib.timed(name[len("hstu_"):], dev):
+        _lib.check(getattr(_lib.lib(), name)(C.byref(p), _lib.stream_ptr(dev)), name)
+    # wgmma path: dK/dV kernel + dQ kernel (d = 32, after the amax and convert kernels for bf16; deterministic d = 64 / 128
+    # and every non-causal call: no workspace, no memset, no convert) or main kernel + dQ convert; generic path: dK/dV
+    # kernel + dQ kernel
     _lib.note_launch(4 if ws is not None and p.dtype == _lib.BF16 and p.dqk == 32 else 2)
     del ws, keep
 
@@ -358,25 +384,25 @@ def _fill_bias(p, bias, dbias):
 class _HSTUAttentionFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
-                min_full_attn_seq_len, impl):
+                min_full_attn_seq_len, impl, causal=True):
         # no Fp16Operands here: q, k, v are saved anyway, so the copies would double the saved bytes to spare only the
         # backward's pre-pass over q, k, v
         out = cuda_hstu_attention_fwd(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
-                                      contextual_seq_len, min_full_attn_seq_len, impl)
+                                      contextual_seq_len, min_full_attn_seq_len, impl, causal=causal)
         ctx.save_for_backward(q, k, v, seq_offsets, num_targets)
-        ctx.args = (max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full_attn_seq_len, impl)
+        ctx.args = (max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full_attn_seq_len, impl, causal)
         return out
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, seq_offsets, num_targets = ctx.saved_tensors
-        max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full, impl = ctx.args
+        max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full, impl, causal = ctx.args
         dq = torch.empty(q.shape, dtype=q.dtype, device=q.device)
         dk = torch.empty(k.shape, dtype=k.dtype, device=k.device)
         dv = torch.empty(v.shape, dtype=v.dtype, device=v.device)
         cuda_hstu_attention_bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, num_targets, max_attn_len,
-                                contextual_seq_len, min_full, impl)
-        return None, None, dq, dk, dv, None, None, None, None, None, None
+                                contextual_seq_len, min_full, impl, causal=causal)
+        return None, None, dq, dk, dv, None, None, None, None, None, None, None
 
 
 def hstu_mha(
@@ -402,7 +428,8 @@ def hstu_mha(
 
     `sort_by_length` and `enable_tma` are accepted for call compatibility: the kernels always schedule heavy tiles
     first and always use TMA where the shape allows.  Precondition (as for the reference Triton backend): every
-    sequence length is <= max_seq_len.
+    sequence length is <= max_seq_len.  causal=False runs the non-causal attention (the reference eager path's
+    causal=False mask), forward and backward.
     """
     _, H, _ = q.shape
     torch._assert(max_seq_len > 0, "max_seq_len must be larger than 0")
@@ -411,11 +438,10 @@ def hstu_mha(
     torch._assert(v.dim() == 3, "v must be 3-D")
     torch._assert(v.shape[0] == q.shape[0], "wrong v shape[0]")
     torch._assert(v.shape[1] == H, "wrong v shape[1]")
-    torch._assert(causal, "only support causal attention")
     require_cuda_kernel(kernel, "hstu_mha")
     torch._assert(dropout_pr < 1e-6, "dropout for the CUDA path is not implemented")
     return _HSTUAttentionFunction.apply(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
-                                        contextual_seq_len, min_full_attn_seq_len, impl)
+                                        contextual_seq_len, min_full_attn_seq_len, impl, bool(causal))
 
 
 def delta_hstu_mha(

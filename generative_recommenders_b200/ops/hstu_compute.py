@@ -184,7 +184,7 @@ class _HSTUPreprocessAndAttentionFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, norm_weight, norm_bias, norm_eps, num_heads, attn_dim, hidden_dim, uvqk_weight, uvqk_bias,
                 max_seq_len, seq_offsets, attn_alpha, num_targets, max_attn_len, contextual_seq_len, recompute_uvqk,
-                recompute_normed_x, impl):
+                recompute_normed_x, impl, causal=True):
         x = _row_major(x)
         normed_x, mean, rstd = cuda_layer_norm_fwd(x, norm_weight, norm_bias, norm_eps, False)
         uvqk = torch.addmm(uvqk_bias, normed_x, uvqk_weight)
@@ -193,22 +193,23 @@ class _HSTUPreprocessAndAttentionFunction(torch.autograd.Function):
         u = cuda_silu_fwd(u_pre)
         # bf16 at dqk == dv == 32: the attention keeps its fp16 copies of q, k, v for the backward, which then needs only u
         # of the uvqk GEMM (L * H * 32 * 2 bytes per copy: memory traded for the q / k / v columns of the recomputed GEMM
-        # and the backward's pre-pass over them)
+        # and the backward's pre-pass over them).  A non-causal attention keeps none, and its backward reads q, k, v.
         ops = Fp16Operands()
         out = cuda_hstu_attention_fwd(max_seq_len, attn_alpha, q.view(-1, H, dqk), k.view(-1, H, dqk), v.view(-1, H, dv),
-                                      seq_offsets, num_targets, max_attn_len, contextual_seq_len, 0, impl, fp16_operands=ops)
+                                      seq_offsets, num_targets, max_attn_len, contextual_seq_len, 0, impl,
+                                      fp16_operands=ops, causal=causal)
         ctx.fp16_operands = ops
         ctx.save_for_backward(x, norm_weight, norm_bias, uvqk_weight, uvqk_bias, mean, rstd, seq_offsets, num_targets,
                               None if recompute_normed_x else normed_x,
                               None if recompute_uvqk else uvqk)
-        ctx.cfg = (norm_eps, H, dqk, dv, max_seq_len, attn_alpha, max_attn_len, contextual_seq_len, impl)
+        ctx.cfg = (norm_eps, H, dqk, dv, max_seq_len, attn_alpha, max_attn_len, contextual_seq_len, impl, causal)
         return u, out.view(-1, H * dv)
 
     @staticmethod
     def backward(ctx, du, dattn):
         (x, norm_weight, norm_bias, uvqk_weight, uvqk_bias, mean, rstd, seq_offsets, num_targets, normed_x,
          uvqk) = ctx.saved_tensors
-        norm_eps, H, dqk, dv, max_seq_len, alpha, max_attn_len, contextual_seq_len, impl = ctx.cfg
+        norm_eps, H, dqk, dv, max_seq_len, alpha, max_attn_len, contextual_seq_len, impl, causal = ctx.cfg
         ops = ctx.fp16_operands
         if normed_x is None:
             normed_x, _, _ = cuda_layer_norm_fwd(x, norm_weight, norm_bias, norm_eps, False, save_stats=False)
@@ -225,14 +226,14 @@ class _HSTUPreprocessAndAttentionFunction(torch.autograd.Function):
         dattn = _row_major(dattn)
         cuda_hstu_attention_bwd(max_seq_len, alpha, dattn.view(-1, H, dv), q, k, v, d_q.view(-1, H, dqk), d_k.view(-1, H, dqk),
                                 d_v.view(-1, H, dv), seq_offsets, num_targets, max_attn_len, contextual_seq_len, 0, impl,
-                                fp16_operands=ops)
+                                fp16_operands=ops, causal=causal)
         cuda_silu_bwd(du, u_pre, d_u)
         d_w = torch.mm(normed_x.t(), duvqk)
         d_b = duvqk.sum(dim=0)
         d_normed = torch.mm(duvqk, uvqk_weight.t())
         dx, dnw, dnb = cuda_layer_norm_bwd(d_normed, x, norm_weight, norm_bias, mean, rstd, False)
         return (dx, dnw.to(norm_weight.dtype), dnb.to(norm_bias.dtype), None, None, None, None, d_w, d_b, None, None, None,
-                None, None, None, None, None, None)
+                None, None, None, None, None, None, None)
 
 
 def hstu_preprocess_and_attention(
@@ -247,13 +248,12 @@ def hstu_preprocess_and_attention(
     torch._assert(x.shape[1] == uvqk_weight.shape[0], "x.shape[1] must equal uvqk_weight.shape[0]")
     torch._assert(uvqk_weight.shape[1] == 2 * num_heads * (hidden_dim + attn_dim),
                   "uvqk_weight.shape[1] must equal 2 * num_heads * (hidden_dim + attn_dim)")
-    torch._assert(causal is True, "only causal attention is supported.")
     require_cuda_kernel(kernel, "hstu_preprocess_and_attention")
     if not prefill:
         u, attn_output = _HSTUPreprocessAndAttentionFunction.apply(
             x, norm_weight, norm_bias, norm_eps, num_heads, attn_dim, hidden_dim, uvqk_weight, uvqk_bias, max_seq_len,
             seq_offsets, attn_alpha, num_targets, max_attn_len, contextual_seq_len, recompute_uvqk_in_backward,
-            recompute_normed_x_in_backward, impl)
+            recompute_normed_x_in_backward, impl, bool(causal))
         return u, attn_output, None, None
     # prefill: the caller needs k and v for the KV cache (hstu_compute.py:230-259)
     u, q, k, v = hstu_compute_uqvk(x, norm_weight, norm_bias, norm_eps, num_heads, attn_dim, hidden_dim, uvqk_weight,

@@ -8,6 +8,8 @@ routes them to libhstu_b200.so, so code written against `torch.ops.hstu.hstu_mha
 
 Arguments this backend does not implement raise instead of being ignored: `attn_scale` and the dense layout
 (`seq_offsets=None`).
+`causal=False` (the reference CUDA op's default) runs the non-causal attention under the reference eager path's
+causal=False mask (ops/hstu_attention.py `causal=False`), forward and backward; it takes no fp8 inputs.
 fp8: with q, k and v of dtype float8_e4m3fn, `hstu_mha_fwd` and `hstu_mha` run the fp8 forward (`hstu_attn_fwd_fp8`) and
 return bf16: the attention of q * q_descale[b, h], k * k_descale[b, h], v * v_descale[b, h], each descale an fp32 [B, H]
 tensor or None for 1, as in the reference's e4m3 forward.  Head dims: dqk == dv, or dqk < dv (the DLRM-HSTU default
@@ -42,7 +44,6 @@ _FP8 = torch.float8_e4m3fn
 
 
 def _check(causal, seq_offsets, attn_scale, descales, qkv=()):
-    torch._assert(causal, "only support causal attention")
     if seq_offsets is None:
         raise RuntimeError("hstu::hstu_mha on H100: the dense (seq_offsets=None) layout is not implemented; pass jagged tensors")
     if attn_scale is not None:
@@ -57,14 +58,16 @@ def _fwd(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_sca
     descales = (q_descale, k_descale, v_descale)
     _check(causal, seq_offsets, attn_scale, descales, (q, k, v))
     return cuda_hstu_attention_fwd(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
-                                   min_full_attn_seq_len, descales=descales if any(t.dtype == _FP8 for t in (q, k, v)) else None)
+                                   min_full_attn_seq_len, descales=descales if any(t.dtype == _FP8 for t in (q, k, v)) else None,
+                                   causal=bool(causal))
 
 
 def _bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, causal, num_targets, attn_scale, max_attn_len,
          min_full_attn_seq_len, contextual_seq_len, sort_by_length, deterministic, sm_margin) -> List[torch.Tensor]:
     _check(causal, seq_offsets, attn_scale, ())
     cuda_hstu_attention_bwd(int(max_seq_len), alpha, dout, q, k, v, dq, dk, dv, seq_offsets, num_targets, max_attn_len,
-                            contextual_seq_len, min_full_attn_seq_len, deterministic=_deterministic(deterministic))
+                            contextual_seq_len, min_full_attn_seq_len, deterministic=_deterministic(deterministic),
+                            causal=bool(causal))
     return [dq, dk, dv]
 
 
@@ -75,20 +78,22 @@ def _deterministic(flag):
 
 class _Mha(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, min_full, ctx_len, deterministic):
-        out = cuda_hstu_attention_fwd(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, ctx_len, min_full)
+    def forward(ctx, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, min_full, ctx_len, deterministic,
+                causal=True):
+        out = cuda_hstu_attention_fwd(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, ctx_len, min_full,
+                                      causal=causal)
         ctx.save_for_backward(q, k, v, seq_offsets, num_targets)
-        ctx.cfg = (max_seq_len, alpha, max_attn_len, min_full, ctx_len, deterministic)
+        ctx.cfg = (max_seq_len, alpha, max_attn_len, min_full, ctx_len, deterministic, causal)
         return out
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, seq_offsets, num_targets = ctx.saved_tensors
-        max_seq_len, alpha, max_attn_len, min_full, ctx_len, deterministic = ctx.cfg
+        max_seq_len, alpha, max_attn_len, min_full, ctx_len, deterministic, causal = ctx.cfg
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
         cuda_hstu_attention_bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, num_targets, max_attn_len, ctx_len,
-                                min_full, deterministic=_deterministic(deterministic))
-        return None, None, dq, dk, dv, None, None, None, None, None, None
+                                min_full, deterministic=_deterministic(deterministic), causal=causal)
+        return None, None, dq, dk, dv, None, None, None, None, None, None, None
 
 
 def _mha(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_scale, max_attn_len, min_full_attn_seq_len,
@@ -100,9 +105,9 @@ def _mha(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_sca
             raise RuntimeError("hstu::hstu_mha on H100: fp8 attention is forward only (the reference has no fp8 backward); "
                                "run it under torch.no_grad() or on tensors that do not require grad")
         return cuda_hstu_attention_fwd(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
-                                       contextual_seq_len, min_full_attn_seq_len, descales=descales)
+                                       contextual_seq_len, min_full_attn_seq_len, descales=descales, causal=bool(causal))
     return _Mha.apply(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len, min_full_attn_seq_len,
-                      contextual_seq_len, bool(deterministic))
+                      contextual_seq_len, bool(deterministic), bool(causal))
 
 
 def _fwd_meta(max_seq_len, alpha, q, k, v, *args):

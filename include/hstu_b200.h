@@ -30,6 +30,8 @@
  *        ops/jagged_tensors.py:210-253, ops/pytorch/pt_jagged.py:77-98, ops/triton/triton_jagged.py:56-347
  *   hstu_sampled_softmax_fwd / _bwd
  *        research/modeling/sequential/losses/sampled_softmax.py:29-193, autoregressive_losses.py:73-121
+ *   hstu_attn_fwd_bidir / hstu_attn_bwd_bidir (causal=False)
+ *        ops/hstu_attention.py:44-128 hstu_mha(causal=False); ops/pytorch/pt_hstu_attention.py:33-84 (the mask)
  *   hstu_mask_valid / hstu_kv_tile_range (host-side helpers, no GPU needed)
  *        ops/pytorch/pt_hstu_attention.py:33-84 (_get_valid_attn_mask)
  */
@@ -186,6 +188,20 @@ size_t hstu_attn_fp8_kv_workspace_bytes(const hstu_attn_params* p);
  * device, and hstu_attn_fwd_fp8 itself then returns HSTU_ERR_UNSUPPORTED on a device other than sm_90. */
 int hstu_attn_select_impl(const hstu_attn_params* p, int is_backward);
 
+/* Non-causal (causal=False) attention: hstu_attn_fwd / hstu_attn_bwd under the reference eager path's causal=False mask
+ * (pt_hstu_attention.py:33-84): with the ids of the causal mask, dist = |id_i - id_j|, valid = (i == j) | (dist > 0), then
+ * max_attn_len / min_full_attn_seq_len on dist and the contextual rule.  History rows see the target keys; a target row
+ * sees every history key (within the window) and of the target keys only its own.  Same params and semantics otherwise
+ * (alpha, 1 / max_seq_len, rows >= max_seq_len zero).  HSTU_ERR_UNSUPPORTED for delta_q_len > 0, a relative bias or
+ * HSTU_E4M3.  The wgmma kernels take bf16 / fp16 at dqk == dv in {32, 64, 128} (the backward: atomic-free dK / dV and dQ
+ * kernels at every dim, so it is bitwise reproducible whatever `deterministic` says); everything else runs the generic
+ * kernels.  hstu_attn_bidir_select_impl / hstu_attn_bidir_workspace_bytes answer as hstu_attn_select_impl /
+ * hstu_attn_workspace_bytes do for the causal calls. */
+int hstu_attn_fwd_bidir(const hstu_attn_params* p, void* cuda_stream);
+int hstu_attn_bwd_bidir(const hstu_attn_params* p, void* cuda_stream);
+size_t hstu_attn_bidir_workspace_bytes(const hstu_attn_params* p, int is_backward);
+int hstu_attn_bidir_select_impl(const hstu_attn_params* p, int is_backward);
+
 /* ---- host-side helpers (pure CPU; used by the no-GPU tests to pin the mask / tile-skipping logic) ---- */
 /* 1 if query position i may attend key position j (both < len) -- pt_hstu_attention.py:33-84. */
 int hstu_mask_valid(int32_t len, int32_t num_targets /* <0: none */, int32_t max_attn_len,
@@ -197,6 +213,15 @@ int hstu_kv_range_for_q_rows(int32_t len, int32_t num_targets, int32_t max_attn_
 int hstu_q_range_for_kv_rows(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
                              int32_t contextual_seq_len, int32_t n0, int32_t n1, int32_t* lo, int32_t* hi,
                              int32_t* ctx_hi);
+
+/* The same under the non-causal mask (hstu_attn_fwd_bidir).  Without max_attn_len both ranges are [0, len). */
+int hstu_mask_valid_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
+                          int32_t contextual_seq_len, int32_t i, int32_t j);
+int hstu_kv_range_for_q_rows_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
+                                   int32_t contextual_seq_len, int32_t m0, int32_t m1, int32_t* lo, int32_t* hi);
+int hstu_q_range_for_kv_rows_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
+                                   int32_t contextual_seq_len, int32_t n0, int32_t n1, int32_t* lo, int32_t* hi,
+                                   int32_t* ctx_hi);
 
 /* ---- row-wise normalisation (HBM-bound) ---- */
 /* y = LN(x) * w + b (w,b nullable); swish != 0: y = x * sigmoid(LN(x)*w+b).  mean/rstd [n_rows] fp32 saved for bwd

@@ -26,7 +26,8 @@ import tempfile
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 CSRC = os.path.join(ROOT, "generative_recommenders_b200", "csrc")
 UNITS = ("attn_wgmma_fwd.cu", "attn_wgmma_bwd.cu", "attn_wgmma_fwd_e4m3.cu", "attn_wgmma_mixed_fwd.cu", "attn_wgmma_mixed_bwd.cu",
-         "attn_wgmma_mixed_fwd_e4m3.cu", "attn_wgmma_delta_fp8kv.cu")
+         "attn_wgmma_mixed_fwd_e4m3.cu", "attn_wgmma_delta_fp8kv.cu",
+         "attn_wgmma_bidir.cu")
 _CTRL = ("BRA", "BRX", "JMP", "JMX", "CALL", "RET", "EXIT", "BSSY")  # instructions that end a block or name a branch target
 
 
