@@ -4,6 +4,11 @@
 // cast back to the dtype of `jagged`), ops/triton/triton_jagged.py:56-347 (kernels + backward).
 // Here: fp32-accumulate tiles on the CUDA cores (64 x 64 outputs per CTA, 4 x 4 per thread, K in steps of 16): the only caller
 // (modules/contextualize_mlps.py:136) runs it once per batch outside the STU stack with K, N = a few hundred.
+// Rows at positions >= max_seq_len of a sequence are written as exact zeros (the eager path truncates the padded operand at
+// max_seq_len and dense_to_jagged pads those rows with 0); so they pass no gradient to jagged either (the d_jagged pass is the
+// same kernel), and the wgrad kernel reads no row past max_seq_len.  The grid has ceil(max_seq_len / 64) row tiles per
+// sequence, as the reference's; a CTA strides over its sequence's tiles by that count, so every row of a longer sequence is
+// written without the host learning the longest length.
 //   forward / d_jagged:  C[r, n] = sum_k A[r, k] * B[b][k, n]   (TRANS_B: B[b][n, k])   (+ bias[b, n])
 //   d_dense / d_bias:    dW[b][k, n] = sum_{r in b} A[r, k] * G[r, n];   dbias[b, n] = sum_{r in b} G[r, n]
 #include "common.cuh"
@@ -21,56 +26,58 @@ __global__ void __launch_bounds__(256) jagged_bmm_kernel(const T* __restrict__ A
   const int b = blockIdx.z;
   const long long r0 = load_index(offsets, off_i64, b);
   long long len = load_index(offsets, off_i64, b + 1) - r0;
-  const int m0 = blockIdx.x * 64, n0 = blockIdx.y * 64;
-  if (m0 >= len) return;
+  const int n0 = blockIdx.y * 64;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const bool live = m0 < max_seq_len;  // rows >= max_seq_len are dropped by the padded eager path and come back as zeros
-  float acc[4][4] = {};
   const T* Bb = Bm + (long long)b * K * N;
-  if (live) {
-    for (int k0 = 0; k0 < K; k0 += 16) {
-      for (int idx = tid; idx < 64 * 16; idx += 256) {
-        const int r = idx >> 4, k = idx & 15;   // A tile: 64 rows x 16 k
-        const long long row = m0 + r;
-        float v = 0.f;
-        if (row < len && row < max_seq_len && k0 + k < K) v = Cvt<T>::to_f(A[(r0 + row) * K + k0 + k]);
-        sA[k][r] = v;
+  // m0 and len are uniform across the CTA, so the barriers below are too
+  for (long long m0 = (long long)blockIdx.x * 64; m0 < len; m0 += (long long)gridDim.x * 64) {
+    const bool live = m0 < max_seq_len;  // tiles at or past max_seq_len only store zeros
+    float acc[4][4] = {};
+    if (live) {
+      for (int k0 = 0; k0 < K; k0 += 16) {
+        for (int idx = tid; idx < 64 * 16; idx += 256) {
+          const int r = idx >> 4, k = idx & 15;   // A tile: 64 rows x 16 k
+          const long long row = m0 + r;
+          float v = 0.f;
+          if (row < len && row < max_seq_len && k0 + k < K) v = Cvt<T>::to_f(A[(r0 + row) * K + k0 + k]);
+          sA[k][r] = v;
+        }
+        for (int idx = tid; idx < 64 * 16; idx += 256) {
+          int k, n;
+          if (TRANS_B) { n = idx >> 4; k = idx & 15; } else { k = idx >> 6; n = idx & 63; }
+          float v = 0.f;
+          if (k0 + k < K && n0 + n < N)
+            v = Cvt<T>::to_f(TRANS_B ? Bb[(long long)(n0 + n) * K + k0 + k] : Bb[(long long)(k0 + k) * N + n0 + n]);
+          sB[k][n] = v;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+          float a[4], bb[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) a[i] = sA[k][ty * 4 + i];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) bb[j] = sB[k][tx * 4 + j];
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] += a[i] * bb[j];
+        }
+        __syncthreads();
       }
-      for (int idx = tid; idx < 64 * 16; idx += 256) {
-        int k, n;
-        if (TRANS_B) { n = idx >> 4; k = idx & 15; } else { k = idx >> 6; n = idx & 63; }
-        float v = 0.f;
-        if (k0 + k < K && n0 + n < N)
-          v = Cvt<T>::to_f(TRANS_B ? Bb[(long long)(n0 + n) * K + k0 + k] : Bb[(long long)(k0 + k) * N + n0 + n]);
-        sB[k][n] = v;
-      }
-      __syncthreads();
-#pragma unroll
-      for (int k = 0; k < 16; ++k) {
-        float a[4], bb[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) a[i] = sA[k][ty * 4 + i];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) bb[j] = sB[k][tx * 4 + j];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[i][j] += a[i] * bb[j];
-      }
-      __syncthreads();
     }
-  }
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const long long row = m0 + ty * 4 + i;
-    if (row >= len) continue;
+    for (int i = 0; i < 4; ++i) {
+      const long long row = m0 + ty * 4 + i;
+      if (row >= len) continue;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + tx * 4 + j;
-      if (n >= N) continue;
-      float v = 0.f;
-      if (row < max_seq_len) v = acc[i][j] + (bias ? Cvt<T>::to_f(bias[(long long)b * N + n]) : 0.f);
-      C[(r0 + row) * N + n] = Cvt<T>::from_f(v);
+      for (int j = 0; j < 4; ++j) {
+        const int n = n0 + tx * 4 + j;
+        if (n >= N) continue;
+        float v = 0.f;
+        if (row < max_seq_len) v = acc[i][j] + (bias ? Cvt<T>::to_f(bias[(long long)b * N + n]) : 0.f);
+        C[(r0 + row) * N + n] = Cvt<T>::from_f(v);
+      }
     }
   }
 }

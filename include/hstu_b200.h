@@ -296,11 +296,13 @@ int hstu_position_embeddings_bwd(const void* dout, void* d_seq_embeddings, float
 
 /* out[rows of sequence b] = jagged[rows of b] @ dense[b] + bias[b]  (ops/jagged_tensors.py:210-253, ops/pytorch/pt_jagged.py:77-98):
  * jagged [L, K], dense [B, K, N] (or [B, N, K] with dense_is_transposed: the d_jagged = dout @ dense^T pass), bias [B, N] or NULL,
- * out [L, N]; fp32 accumulation, result in `dtype`.  Rows at positions >= max_seq_len of a sequence are written as zeros.     */
+ * out [L, N]; fp32 accumulation, result in `dtype`.  Every row is written, however long its sequence: rows at positions
+ * >= max_seq_len of a sequence are exact zeros (the eager path truncates at max_seq_len and pads those rows with 0).          */
 int hstu_jagged_dense_bmm_broadcast_add(const void* jagged, const void* dense, const void* bias, void* out,
                                         const void* seq_offsets, int32_t offsets_are_i64, int32_t batch, int32_t K, int32_t N,
                                         int32_t max_seq_len, int32_t dense_is_transposed, int32_t dtype, void* cuda_stream);
-/* d_dense[b] = jagged[rows of b]^T @ dout[rows of b]  ([B, K, N]);  d_bias[b] = sum of dout rows of b ([B, N], nullable).      */
+/* d_dense[b] = jagged[rows of b]^T @ dout[rows of b]  ([B, K, N]);  d_bias[b] = sum of dout rows of b ([B, N], nullable);
+ * only the rows at positions < max_seq_len of each sequence take part, as in the forward.                                   */
 int hstu_jagged_dense_bmm_wgrad(const void* jagged, const void* dout, void* d_dense, void* d_bias, const void* seq_offsets,
                                 int32_t offsets_are_i64, int32_t batch, int32_t K, int32_t N, int32_t max_seq_len, int32_t dtype,
                                 void* cuda_stream);

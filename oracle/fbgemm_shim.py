@@ -55,11 +55,16 @@ def _dense_to_jagged(
     x_offsets: List[torch.Tensor],
     total_L: Optional[int] = None,
 ) -> Tuple[torch.Tensor, List[torch.Tensor]]:
-    # dense [B, N, D] -> values [L, D] taking the first len_b rows of each batch entry.
+    # dense [B, N, D] -> values [L, D] taking the first len_b rows of each batch entry.  A jagged row past the dense length
+    # (len_b > N) gets the padding value 0, as fbgemm writes it, so that there are always offsets[-1] rows.
     assert len(x_offsets) == 1
     off = x_offsets[0].to(torch.int64)
     B, N = dense.shape[0], dense.shape[1]
     lengths = off[1:] - off[:-1]
+    longest = int(lengths.max()) if B > 0 else 0
+    if longest > N:
+        dense = torch.cat([dense, dense.new_zeros((B, longest - N) + tuple(dense.shape[2:]))], dim=1)
+        N = longest
     pos = torch.arange(N, device=dense.device).view(1, N)
     valid = pos < lengths.view(B, 1)
     values = dense.reshape(B * N, -1)[valid.reshape(-1)]

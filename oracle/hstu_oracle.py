@@ -432,12 +432,16 @@ def position_indices(seq_offsets, seq_lengths, timestamps, num_targets, max_cont
 
 
 def add_timestamp_positional_embeddings(alpha, max_contextual_seq_len, pos_w, ts_w, seq_offsets, seq_lengths, seq_embeddings,
-                                        timestamps, num_targets, interleave_targets, time_bucket_fn, dout=None):
+                                        timestamps, num_targets, interleave_targets, time_bucket_fn, dout=None,
+                                        num_time_buckets=None):
     """out = (seq * alpha) + (pos_w[pos] + ts_w[bucket]).to(dtype) with the reference's roundings (position.py:58,
-    pt_position.py:124-133); with `dout`: also (d_seq, d_pos_w, d_ts_w) = (dout * alpha, scatter-adds of dout in fp32)."""
+    pt_position.py:124-133); with `dout`: also (d_seq, d_pos_w, d_ts_w) = (dout * alpha, scatter-adds of dout in fp32).
+    num_time_buckets: the bucket clamp, ts_w.size(1) - 1 as the eager path has it unless given (the CUDA facade passes
+    min(ts_w.size(1), ts_w.size(0)) - 1 so that a table with fewer rows than columns is not indexed past its end)."""
     dt = seq_embeddings.dtype
+    nb = ts_w.shape[1] - 1 if num_time_buckets is None else num_time_buckets
     pos, bkt = position_indices(seq_offsets, seq_lengths, timestamps, num_targets, max_contextual_seq_len, pos_w.shape[0],
-                                ts_w.shape[1] - 1, interleave_targets, time_bucket_fn)
+                                nb, interleave_targets, time_bucket_fn)
     emb = (ts_w.float()[bkt] + pos_w.float()[pos]).to(dt)
     out = (seq_embeddings * alpha) + emb
     if dout is None:
@@ -454,15 +458,21 @@ def add_timestamp_positional_embeddings(alpha, max_contextual_seq_len, pos_w, ts
 
 
 def jagged_dense_bmm_broadcast_add(max_seq_len, seq_offsets, jagged, dense, bias):
-    """out[rows of b] = jagged[rows of b] @ dense[b] + bias[b], operands promoted to fp32 and the result cast back to the dtype
-    of `jagged` (pt_jagged.py:84-97); one sequence at a time (exact: sequences are independent).  Differentiable (autograd)."""
+    """out[rows of b] = jagged[rows of b] @ dense[b] + bias[b], operands promoted to fp32 (fp64 stays fp64) and the result cast
+    back to the dtype of `jagged` (pt_jagged.py:84-97); one sequence at a time (exact: sequences are independent).  Rows at
+    positions >= max_seq_len of a sequence are exact zeros, not the bias: the eager path truncates the padded operand at
+    max_seq_len and dense_to_jagged pads those rows with 0.  So they also pass no gradient.  Differentiable (autograd)."""
     off = _lens(seq_offsets)
+    ct = torch.promote_types(jagged.dtype, torch.float32)
     outs = []
     for b in range(len(off) - 1):
         s, e = int(off[b]), int(off[b + 1])
-        rows = jagged[s:e].to(torch.float32)
-        outs.append(rows @ dense[b].to(torch.float32) + bias[b].to(torch.float32).unsqueeze(0))
-    out = torch.cat(outs, dim=0) if outs else jagged.new_zeros((0, dense.shape[2]), dtype=torch.float32)
+        m = max(0, min(e - s, int(max_seq_len)))
+        rows = jagged[s:s + m].to(ct)
+        outs.append(rows @ dense[b].to(ct) + bias[b].to(ct).unsqueeze(0))
+        if e - s > m:
+            outs.append(jagged.new_zeros((e - s - m, dense.shape[2]), dtype=ct))
+    out = torch.cat(outs, dim=0) if outs else jagged.new_zeros((0, dense.shape[2]), dtype=ct)
     return out.to(jagged.dtype)
 
 

@@ -350,13 +350,19 @@ def ssl_case(name, seed, B, N, D, R, V, l2_norm, temperature, dtype):
                os.path.join(HERE, f"ssl_{name}.pt"))
 
 
-def jagged_bmm_case(name, seed, B, max_len, K, N, dtype):
-    # ops/tests/jagged_tensors_test.py:_test_jagged_dense_bmm_broadcast_add recipe; eager path ops/pytorch/pt_jagged.py:77-98
+def jagged_bmm_case(name, seed, B, max_len, K, N, dtype, lengths=None):
+    # ops/tests/jagged_tensors_test.py:_test_jagged_dense_bmm_broadcast_add recipe; eager path ops/pytorch/pt_jagged.py:77-98.
+    # `lengths` given: those sequence lengths instead of random ones up to max_len (the eager path truncates at max_len and
+    # dense_to_jagged pads the rows past it with 0)
     from generative_recommenders.ops.jagged_tensors import jagged_dense_bmm_broadcast_add
 
     g = torch.Generator().manual_seed(seed)
-    lengths = torch.randint(max_len + 1, (B,), generator=g)
-    lengths[0] = 0
+    if lengths is None:
+        lengths = torch.randint(max_len + 1, (B,), generator=g)
+        lengths[0] = 0
+    else:
+        lengths = torch.tensor(lengths, dtype=torch.int64)
+        B = lengths.numel()
     off = offsets_from(lengths.tolist())
     L = int(off[-1])
     jag = torch.empty(L, K).uniform_(-1, 1, generator=g).to(dtype).requires_grad_()
@@ -421,6 +427,9 @@ def main():
     if not only or "jagged_bmm" in only:
         jagged_bmm_case("f32", 95, 5, 40, 24, 36, torch.float32)
         jagged_bmm_case("bf16", 96, 4, 70, 64, 80, torch.bfloat16)
+    if not only or "jagged_bmm_past_max_len" in only:
+        # sequences longer than max_seq_len, which is not a multiple of the 64-row tile
+        jagged_bmm_case("past_max_len_bf16", 97, 0, 100, 24, 40, torch.bfloat16, lengths=[0, 100, 101, 129, 300, 37, 0])
     if not only or "ssl" in only:
         ssl_case("l2_f32", 91, 4, 12, 64, 16, 50, True, 0.05, torch.float32)
         ssl_case("plain_f32", 92, 3, 9, 32, 8, 40, False, 1.0, torch.float32)
