@@ -59,9 +59,25 @@ int bind_device(const void* ptr) {
   return 0;
 }
 
-// A deterministic backward takes the same route as any other: the wgmma kernels run their atomic-free split path
-// (attn_wgmma_bwd.cu), and the generic kernels have no atomics on q / k / v.
-static int select_impl(const hstu_attn_params* p, bool bwd) {
+// Which kernels take a call: HSTU_IMPL_UMMA (the wgmma kernels), HSTU_IMPL_GENERIC, or a refusal.  bidir: the non-causal
+// mask, whose kernels take no delta-q, relative bias or e4m3 input (the reference's KV-cached path is causal, and there is no
+// fp8 backward).  A deterministic backward takes the same route as any other: the wgmma kernels run their atomic-free split
+// path (attn_wgmma_bwd.cu), and the generic kernels have no atomics on q / k / v.
+static int select_impl(const hstu_attn_params* p, bool bwd, bool bidir) {
+  if (bidir) {
+    if (p->delta_q_len > 0) {
+      set_error("non-causal attention: delta_q (the KV-cached forward) is causal only");
+      return HSTU_ERR_UNSUPPORTED;
+    }
+    if (p->pos_w != nullptr || p->ts_w != nullptr) {
+      set_error("non-causal attention: the relative bias is not supported");
+      return HSTU_ERR_UNSUPPORTED;
+    }
+    if (p->dtype == HSTU_E4M3) {
+      set_error("non-causal attention: fp8 (e4m3) inputs are not supported");
+      return HSTU_ERR_UNSUPPORTED;
+    }
+  }
   if (p->dtype == HSTU_E4M3) {  // the fp8 forward: wgmma kernels only, whatever the device (hstu_attn_fwd_fp8 checks it)
     if (bwd) {
       set_error("fp8 (e4m3) attention has no backward: hstu_attn_fwd_fp8 is a forward-only entry");
@@ -79,41 +95,16 @@ static int select_impl(const hstu_attn_params* p, bool bwd) {
               "with atomics");
     return HSTU_ERR_UNSUPPORTED;
   }
-  const bool can = wgmma_supported(*p, bwd);
+  const bool can = wgmma_supported(*p, bwd, bidir);
   if (p->impl == HSTU_IMPL_GENERIC) return HSTU_IMPL_GENERIC;
   if (p->impl == HSTU_IMPL_UMMA) {
     if (!can) {
-      set_error("wgmma path does not support this problem (dtype=%d dqk=%d dv=%d delta=%d bias=%d)", p->dtype, p->dqk,
-                p->dv, p->delta_q_len, p->pos_w != nullptr || p->ts_w != nullptr);
-      return HSTU_ERR_UNSUPPORTED;
-    }
-    return HSTU_IMPL_UMMA;
-  }
-  return can ? HSTU_IMPL_UMMA : HSTU_IMPL_GENERIC;
-}
-
-// The non-causal entry points (hstu_attn_fwd_bidir / hstu_attn_bwd_bidir): the routing of select_impl with the support check
-// of the non-causal wgmma kernels (attn_wgmma_bidir.cu).  The reference's KV-cached path is causal, and there is no fp8
-// backward: delta-q, a relative bias and e4m3 inputs are refused.
-static int select_impl_bidir(const hstu_attn_params* p, bool bwd) {
-  if (p->delta_q_len > 0) {
-    set_error("non-causal attention: delta_q (the KV-cached forward) is causal only");
-    return HSTU_ERR_UNSUPPORTED;
-  }
-  if (p->pos_w != nullptr || p->ts_w != nullptr) {
-    set_error("non-causal attention: the relative bias is not supported");
-    return HSTU_ERR_UNSUPPORTED;
-  }
-  if (p->dtype == HSTU_E4M3) {
-    set_error("non-causal attention: fp8 (e4m3) inputs are not supported");
-    return HSTU_ERR_UNSUPPORTED;
-  }
-  const bool can = wgmma_bidir_supported(*p, bwd);
-  if (p->impl == HSTU_IMPL_GENERIC) return HSTU_IMPL_GENERIC;
-  if (p->impl == HSTU_IMPL_UMMA) {
-    if (!can) {
-      set_error("non-causal wgmma path does not support this problem (dtype=%d dqk=%d dv=%d): it takes bf16 / fp16 at "
-                "dqk == dv in {32, 64, 128}; d = 256, dqk != dv and fp32 run on the generic kernels", p->dtype, p->dqk, p->dv);
+      if (bidir)
+        set_error("non-causal wgmma path does not support this problem (dtype=%d dqk=%d dv=%d): it takes bf16 / fp16 at "
+                  "dqk == dv in {32, 64, 128}; d = 256, dqk != dv and fp32 run on the generic kernels", p->dtype, p->dqk, p->dv);
+      else
+        set_error("wgmma path does not support this problem (dtype=%d dqk=%d dv=%d delta=%d bias=%d)", p->dtype, p->dqk,
+                  p->dv, p->delta_q_len, p->pos_w != nullptr || p->ts_w != nullptr);
       return HSTU_ERR_UNSUPPORTED;
     }
     return HSTU_IMPL_UMMA;
@@ -123,7 +114,42 @@ static int select_impl_bidir(const hstu_attn_params* p, bool bwd) {
 
 // The calls that run on scaled fp16 operands (attn_fp16_operands.cu): those of runs_on_fp16_operands on the wgmma kernels
 static bool wgmma_on_fp16_operands(const hstu_attn_params* p, bool bwd) {
-  return runs_on_fp16_operands(*p) && select_impl(p, bwd) == HSTU_IMPL_UMMA;
+  return runs_on_fp16_operands(*p) && select_impl(p, bwd, false) == HSTU_IMPL_UMMA;
+}
+
+// The bodies of hstu_attn_select_impl, _workspace_bytes, _fwd and _bwd and of their non-causal twins (bidir)
+static int checked_select_impl(const hstu_attn_params* p, bool bwd, bool bidir) {
+  if (int e = validate_attn(p, bwd)) return e;
+  return select_impl(p, bwd, bidir);
+}
+
+static size_t workspace_bytes(const hstu_attn_params* p, bool bwd, bool bidir) {
+  if (p == nullptr || validate_attn(p, bwd) != 0 || p->batch == 0 || p->total_rows == 0) return 0;
+  if (select_impl(p, bwd, bidir) != HSTU_IMPL_UMMA) return 0;
+  return p->dtype == HSTU_E4M3 ? e4m3_v_copy_bytes(*p) : wgmma_workspace_bytes(*p, bwd, bidir);  // e4m3: the fp16 copy of v
+}
+
+// The causal entries refuse e4m3 themselves, return 0 on an empty problem (triton_hstu_attention.py:1789-1790) and bind the
+// device of q before routing; the non-causal ones route first, so their refusals come before all three.
+static int run_attn(const hstu_attn_params* p, bool bwd, bool bidir, cudaStream_t st) {
+  if (int e = validate_attn(p, bwd)) return e;
+  if (!bidir && p->dtype == HSTU_E4M3) {
+    if (!bwd) {
+      set_error("hstu_attn_fwd: fp8 (e4m3) inputs go through hstu_attn_fwd_fp8 (with their descales)");
+      return HSTU_ERR_INVALID_ARGUMENT;
+    }
+    set_error("hstu_attn_bwd: fp8 (e4m3) attention has no backward (hstu_attn_fwd_fp8 is forward only)");
+    return HSTU_ERR_UNSUPPORTED;
+  }
+  int impl = bidir ? select_impl(p, bwd, true) : 0;
+  if (impl < 0) return impl;
+  if (p->batch == 0 || p->total_rows == 0) return 0;
+  if (int e = bind_device(p->q)) return e;
+  if (!bidir) impl = select_impl(p, bwd, false);
+  if (impl < 0) return impl;
+  if (impl == HSTU_IMPL_GENERIC) return bwd ? attn_generic_bwd(*p, st, bidir) : attn_generic_fwd(*p, st, bidir);
+  if (bidir) return bwd ? attn_wgmma_bidir_bwd(*p, st) : attn_wgmma_bidir_fwd(*p, st);
+  return bwd ? attn_wgmma_bwd(*p, st) : attn_wgmma_fwd(*p, st);
 }
 
 // Nullable descales: no negative strides, fp32-aligned pointers.
@@ -160,6 +186,38 @@ static int check_descale_devices(const hstu_attn_descales* d) {
   return 0;
 }
 
+// The bodies of the mask exports (hstu_mask_valid, hstu_kv_range_for_q_rows, hstu_q_range_for_kv_rows) and of their
+// non-causal twins (bidir)
+static int seq_mask_valid(bool bidir, int len, int num_targets, int max_attn_len, int min_full, int ctx, int i, int j) {
+  const SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full, ctx);
+  return (bidir ? mask_valid_bidir(m, i, j) : mask_valid(m, i, j)) ? 1 : 0;
+}
+
+static int kv_range(bool bidir, int len, int num_targets, int max_attn_len, int min_full, int ctx, int m0, int m1, int32_t* lo,
+                    int32_t* hi) {
+  HSTU_CHECK_ARG(lo && hi && m0 >= 0 && m1 > m0 && m1 <= len, "bad row range");
+  const SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full, ctx);
+  int l, h;
+  if (bidir) kv_range_for_q_rows_bidir(m, m0, m1, &l, &h);
+  else kv_range_for_q_rows(m, m0, m1, &l, &h);
+  *lo = l;
+  *hi = h;
+  return 0;
+}
+
+static int q_range(bool bidir, int len, int num_targets, int max_attn_len, int min_full, int ctx, int n0, int n1, int32_t* lo,
+                   int32_t* hi, int32_t* ctx_hi) {
+  HSTU_CHECK_ARG(lo && hi && ctx_hi && n0 >= 0 && n1 > n0 && n1 <= len, "bad row range");
+  const SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full, ctx);
+  int l, h, c;
+  if (bidir) q_range_for_kv_rows_bidir(m, n0, n1, &l, &h, &c);
+  else q_range_for_kv_rows(m, n0, n1, &l, &h, &c);
+  *lo = l;
+  *hi = h;
+  *ctx_hi = c;
+  return 0;
+}
+
 }  // namespace hstu
 
 using namespace hstu;
@@ -169,82 +227,21 @@ extern "C" {
 const char* hstu_last_error(void) { return g_err; }
 int hstu_abi_version(void) { return HSTU_B200_ABI_VERSION; }
 
-int hstu_attn_select_impl(const hstu_attn_params* p, int is_backward) {
-  if (int e = validate_attn(p, is_backward != 0)) return e;
-  return select_impl(p, is_backward != 0);
-}
+int hstu_attn_select_impl(const hstu_attn_params* p, int is_backward) { return checked_select_impl(p, is_backward != 0, false); }
+size_t hstu_attn_workspace_bytes(const hstu_attn_params* p, int is_backward) { return workspace_bytes(p, is_backward != 0, false); }
+int hstu_attn_fwd(const hstu_attn_params* p, void* stream) { return run_attn(p, false, false, (cudaStream_t)stream); }
+int hstu_attn_bwd(const hstu_attn_params* p, void* stream) { return run_attn(p, true, false, (cudaStream_t)stream); }
 
-size_t hstu_attn_workspace_bytes(const hstu_attn_params* p, int is_backward) {
-  if (p == nullptr) return 0;
-  if (validate_attn(p, is_backward != 0) != 0) return 0;
-  if (p->batch == 0 || p->total_rows == 0) return 0;
-  int impl = select_impl(p, is_backward != 0);
-  if (p->dtype == HSTU_E4M3) return impl == HSTU_IMPL_UMMA ? e4m3_v_copy_bytes(*p) : 0;  // the fp16 copy of v
-  if (impl == HSTU_IMPL_UMMA) return wgmma_workspace_bytes(*p, is_backward != 0);
-  return 0;
-}
-
-int hstu_attn_fwd(const hstu_attn_params* p, void* stream) {
-  if (int e = validate_attn(p, false)) return e;
-  HSTU_CHECK_ARG(p->dtype != HSTU_E4M3, "hstu_attn_fwd: fp8 (e4m3) inputs go through hstu_attn_fwd_fp8 (with their descales)");
-  if (p->batch == 0 || p->total_rows == 0) return 0;  // triton_hstu_attention.py:1789-1790
-  if (int e = bind_device(p->q)) return e;
-  int impl = select_impl(p, false);
-  if (impl < 0) return impl;
-  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_fwd(*p, (cudaStream_t)stream);
-  return attn_generic_fwd(*p, (cudaStream_t)stream);
-}
-
-int hstu_attn_bwd(const hstu_attn_params* p, void* stream) {
-  if (int e = validate_attn(p, true)) return e;
-  if (p->dtype == HSTU_E4M3) {
-    set_error("hstu_attn_bwd: fp8 (e4m3) attention has no backward (hstu_attn_fwd_fp8 is forward only)");
-    return HSTU_ERR_UNSUPPORTED;
-  }
-  if (p->batch == 0 || p->total_rows == 0) return 0;
-  if (int e = bind_device(p->q)) return e;
-  int impl = select_impl(p, true);
-  if (impl < 0) return impl;
-  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bwd(*p, (cudaStream_t)stream);
-  return attn_generic_bwd(*p, (cudaStream_t)stream);
-}
-
-int hstu_attn_bidir_select_impl(const hstu_attn_params* p, int is_backward) {
-  if (int e = validate_attn(p, is_backward != 0)) return e;
-  return select_impl_bidir(p, is_backward != 0);
-}
-
-size_t hstu_attn_bidir_workspace_bytes(const hstu_attn_params* p, int is_backward) {
-  if (p == nullptr || validate_attn(p, is_backward != 0) != 0) return 0;
-  if (p->batch == 0 || p->total_rows == 0) return 0;
-  return select_impl_bidir(p, is_backward != 0) == HSTU_IMPL_UMMA ? wgmma_bidir_workspace_bytes(*p, is_backward != 0) : 0;
-}
-
-int hstu_attn_fwd_bidir(const hstu_attn_params* p, void* stream) {
-  if (int e = validate_attn(p, false)) return e;
-  const int impl = select_impl_bidir(p, false);
-  if (impl < 0) return impl;
-  if (p->batch == 0 || p->total_rows == 0) return 0;
-  if (int e = bind_device(p->q)) return e;
-  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bidir_fwd(*p, (cudaStream_t)stream);
-  return attn_generic_fwd(*p, (cudaStream_t)stream, true);
-}
-
-int hstu_attn_bwd_bidir(const hstu_attn_params* p, void* stream) {
-  if (int e = validate_attn(p, true)) return e;
-  const int impl = select_impl_bidir(p, true);
-  if (impl < 0) return impl;
-  if (p->batch == 0 || p->total_rows == 0) return 0;
-  if (int e = bind_device(p->q)) return e;
-  if (impl == HSTU_IMPL_UMMA) return attn_wgmma_bidir_bwd(*p, (cudaStream_t)stream);
-  return attn_generic_bwd(*p, (cudaStream_t)stream, true);
-}
+int hstu_attn_bidir_select_impl(const hstu_attn_params* p, int is_backward) { return checked_select_impl(p, is_backward != 0, true); }
+size_t hstu_attn_bidir_workspace_bytes(const hstu_attn_params* p, int is_backward) { return workspace_bytes(p, is_backward != 0, true); }
+int hstu_attn_fwd_bidir(const hstu_attn_params* p, void* stream) { return run_attn(p, false, true, (cudaStream_t)stream); }
+int hstu_attn_bwd_bidir(const hstu_attn_params* p, void* stream) { return run_attn(p, true, true, (cudaStream_t)stream); }
 
 int hstu_attn_fwd_fp8(const hstu_attn_params* p, const hstu_attn_descales* descales, void* stream) {
   if (int e = validate_attn(p, false)) return e;
   HSTU_CHECK_ARG(p->dtype == HSTU_E4M3, "hstu_attn_fwd_fp8: q, k, v must be HSTU_E4M3 (got dtype %d)", p->dtype);
   if (int e = validate_descales(descales)) return e;
-  const int impl = select_impl(p, false);
+  const int impl = select_impl(p, false, false);
   if (impl < 0) return impl;
   if (p->batch == 0 || p->total_rows == 0) return 0;
   if (int e = bind_device(p->q)) return e;
@@ -337,62 +334,34 @@ int hstu_attn_bwd_on_fp16_operands(const hstu_attn_params* p, const void* operan
 
 int hstu_mask_valid(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
                     int32_t contextual_seq_len, int32_t i, int32_t j) {
-  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
-  return mask_valid(m, i, j) ? 1 : 0;
+  return seq_mask_valid(false, len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len, i, j);
 }
 
 int hstu_kv_range_for_q_rows(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
                              int32_t contextual_seq_len, int32_t m0, int32_t m1, int32_t* lo, int32_t* hi) {
-  HSTU_CHECK_ARG(lo && hi && m0 >= 0 && m1 > m0 && m1 <= len, "bad row range");
-  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
-  int l, h;
-  kv_range_for_q_rows(m, m0, m1, &l, &h);
-  *lo = l;
-  *hi = h;
-  return 0;
+  return kv_range(false, len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len, m0, m1, lo, hi);
 }
 
 int hstu_q_range_for_kv_rows(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
                              int32_t contextual_seq_len, int32_t n0, int32_t n1, int32_t* lo, int32_t* hi,
                              int32_t* ctx_hi) {
-  HSTU_CHECK_ARG(lo && hi && ctx_hi && n0 >= 0 && n1 > n0 && n1 <= len, "bad row range");
-  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
-  int l, h, c;
-  q_range_for_kv_rows(m, n0, n1, &l, &h, &c);
-  *lo = l;
-  *hi = h;
-  *ctx_hi = c;
-  return 0;
+  return q_range(false, len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len, n0, n1, lo, hi, ctx_hi);
 }
 
 int hstu_mask_valid_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
                           int32_t contextual_seq_len, int32_t i, int32_t j) {
-  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
-  return mask_valid_bidir(m, i, j) ? 1 : 0;
+  return seq_mask_valid(true, len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len, i, j);
 }
 
 int hstu_kv_range_for_q_rows_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
                                    int32_t contextual_seq_len, int32_t m0, int32_t m1, int32_t* lo, int32_t* hi) {
-  HSTU_CHECK_ARG(lo && hi && m0 >= 0 && m1 > m0 && m1 <= len, "bad row range");
-  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
-  int l, h;
-  kv_range_for_q_rows_bidir(m, m0, m1, &l, &h);
-  *lo = l;
-  *hi = h;
-  return 0;
+  return kv_range(true, len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len, m0, m1, lo, hi);
 }
 
 int hstu_q_range_for_kv_rows_bidir(int32_t len, int32_t num_targets, int32_t max_attn_len, int32_t min_full_attn_seq_len,
                                    int32_t contextual_seq_len, int32_t n0, int32_t n1, int32_t* lo, int32_t* hi,
                                    int32_t* ctx_hi) {
-  HSTU_CHECK_ARG(lo && hi && ctx_hi && n0 >= 0 && n1 > n0 && n1 <= len, "bad row range");
-  SeqMask m = make_seq_mask(len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len);
-  int l, h, c;
-  q_range_for_kv_rows_bidir(m, n0, n1, &l, &h, &c);
-  *lo = l;
-  *hi = h;
-  *ctx_hi = c;
-  return 0;
+  return q_range(true, len, num_targets, max_attn_len, min_full_attn_seq_len, contextual_seq_len, n0, n1, lo, hi, ctx_hi);
 }
 
 int hstu_layer_norm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, int64_t n_rows,

@@ -48,25 +48,22 @@ __global__ void dq_convert_kernel(const float* __restrict__ acc, uint16_t* __res
 // ------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------
-size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd) {
+// bidir: the non-causal kernels take no delta-q, and their backward is always split
+size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd, bool bidir) {
   if (!bwd && p.delta_q_len > 0) return wgmma_delta_workspace_bytes(p);  // the fp32 partials of split key chunks, or 0
   if (runs_on_fp16_operands(p)) return fp16_operands_workspace_bytes(p, bwd);
-  if (!bwd || split_dq(p)) return 0;
+  if (!bwd || bidir || split_dq(p)) return 0;
   return (size_t)p.total_rows * p.heads * p.dqk * sizeof(float);  // fp32 dQ accumulator [L, H, D]
 }
 
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st) {
   if (p.dqk != p.dv) return attn_wgmma_bwd_mixed(p, st);  // split kernels only
   return dispatch_dims(SquareDims{}, p, "wgmma backward", [&]<int D, int, bool BF16>() {
-    if constexpr (scaled_fp16_dims(BF16, D, D)) {  // the fp16 kernels on exactly scaled copies (DESIGN.md 3.0)
-      Fp16Operands f16;
-      if (int e = fp16_operands_prepass(p, true, &f16, st)) return e;
-      return launch_bwd_split<D, D, false>(p, st, attn_bwd_dkdv_wgmma_kernel<D, false>, attn_bwd_dq_wgmma_kernel<D, false>, &f16);
-    } else {
+    return launch_on_operands<D, BF16>(p, true, st, [&]<bool B>(const Fp16Operands* f16) {
       if constexpr (fused_bwd_dims(D, D))
-        if (!split_dq(p)) return launch_bwd_fused<D>(p, st, attn_bwd_wgmma_kernel<D, BF16>, dq_convert_kernel<BF16>);
-      return launch_bwd_split<D, D, BF16>(p, st, attn_bwd_dkdv_wgmma_kernel<D, BF16>, attn_bwd_dq_wgmma_kernel<D, BF16>);
-    }
+        if (!split_dq(p)) return launch_bwd_fused<D>(p, st, attn_bwd_wgmma_kernel<D, B>, dq_convert_kernel<B>);
+      return launch_bwd_split<D, D, B>(p, st, attn_bwd_dkdv_wgmma_kernel<D, B>, attn_bwd_dq_wgmma_kernel<D, B>, f16);
+    });
   });
 }
 

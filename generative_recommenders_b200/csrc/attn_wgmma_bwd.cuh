@@ -704,7 +704,7 @@ template <int D>
 int launch_bwd_fused(const hstu_attn_params& p, cudaStream_t st, void (*kern)(BwdParams),
                      void (*convert)(const float*, uint16_t*, long long, int, int, long long, long long, float)) {
   using Cfg = BwdCfg<D, D, true>;
-  const size_t need = wgmma_workspace_bytes(p, true);
+  const size_t need = wgmma_workspace_bytes(p, true, false);
   if (p.workspace == nullptr || p.workspace_bytes < need) {
     set_error("hstu_attn_bwd: workspace of %zu bytes required (got %zu)", need, p.workspace_bytes);
     return HSTU_ERR_WORKSPACE;

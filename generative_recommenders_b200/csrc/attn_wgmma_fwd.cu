@@ -1,5 +1,5 @@
 // Jagged HSTU attention forward on the wgmma kernels at dqk == dv in {32, 64, 128, 256} (bf16 / fp16), the delta-q reduction,
-// and the routing of every wgmma forward.  The kernel body, its design and its launcher are in attn_wgmma_fwd.cuh; the
+// which calls the wgmma kernels take (causal and non-causal), and the routing of every causal wgmma forward.  The kernel body, its design and its launcher are in attn_wgmma_fwd.cuh; the
 // dqk < dv instantiations are in attn_wgmma_mixed_fwd.cu.
 #include "attn_wgmma_fwd.cuh"
 
@@ -96,7 +96,10 @@ static bool wgmma_bwd_supported(const hstu_attn_params& p) {
          aligned_view(p.dk, p.dk_row_stride, p.dk_head_stride) && aligned_view(p.dv_out, p.dv_row_stride, p.dv_head_stride);
 }
 
-bool wgmma_supported(const hstu_attn_params& p, bool bwd) { return bwd ? wgmma_bwd_supported(p) : wgmma_fwd_supported(p); }
+bool wgmma_supported(const hstu_attn_params& p, bool bwd, bool bidir) {
+  if (bidir && (p.delta_q_len != 0 || !has_dims(BidirDims{}, p.dqk, p.dv))) return false;
+  return bwd ? wgmma_bwd_supported(p) : wgmma_fwd_supported(p);
+}
 
 int launch_delta_reduce(bool bf16, const float* part, void* out, long long rows, int heads, int d, int chunks,
                         long long o_row_stride, long long o_head_stride, float inv_n, cudaStream_t st) {
@@ -113,13 +116,9 @@ int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st) {
   return dispatch_dims(SquareDims{}, p, "wgmma forward", [&]<int D, int, bool BF16>() {
     // bf16 keeps the hi / lo P at d = 32 too: a pre-pass over the whole cache would cost more than it saves
     if (p.delta_q_len > 0) return launch_fwd_wgmma<D, D, BF16, true>(p, st, attn_fwd_delta_wgmma_kernel<D, BF16>);
-    if constexpr (scaled_fp16_dims(BF16, D, D)) {  // the fp16 kernel on exactly scaled copies (DESIGN.md 3.0)
-      Fp16Operands f16;
-      if (int e = fp16_operands_prepass(p, false, &f16, st)) return e;
-      return launch_fwd_wgmma<D, D, false, false>(p, st, attn_fwd_wgmma_kernel<D, false>, &f16);
-    } else {
-      return launch_fwd_wgmma<D, D, BF16, false>(p, st, attn_fwd_wgmma_kernel<D, BF16>);
-    }
+    return launch_on_operands<D, BF16>(p, false, st, [&]<bool B>(const Fp16Operands* f16) {
+      return launch_fwd_wgmma<D, D, B, false>(p, st, attn_fwd_wgmma_kernel<D, B>, f16);
+    });
   });
 }
 

@@ -249,4 +249,19 @@ inline Operands operands(const hstu_attn_params& p, const Fp16Operands* f16) {
   return o;
 }
 
+// Runs launch.template operator()<B>(f16), which launches the kernels of dtype B (bf16 if B) on the operands f16 (null: the
+// inputs).  bf16 at d = 32 runs the fp16 kernels on exactly scaled copies that fp16_operands_prepass writes first (DESIGN.md
+// 3.0); every other call runs the kernels of its own dtype on its inputs.  The bf16 kernels at d = 32 are never named here,
+// so they are never instantiated.
+template <int D, bool BF16, class Launch>
+int launch_on_operands(const hstu_attn_params& p, bool bwd, cudaStream_t st, Launch&& launch) {
+  if constexpr (scaled_fp16_dims(BF16, D, D)) {
+    Fp16Operands f16;
+    if (int e = fp16_operands_prepass(p, bwd, &f16, st)) return e;
+    return launch.template operator()<false>(&f16);
+  } else {
+    return launch.template operator()<BF16>(nullptr);
+  }
+}
+
 }  // namespace hstu

@@ -19,6 +19,8 @@ template <class... Pairs> struct HeadDimList {};
 using SquareDims = HeadDimList<HeadDims<32, 32>, HeadDims<64, 64>, HeadDims<128, 128>, HeadDims<256, 256>>;
 using MixedDims = HeadDimList<HeadDims<32, 64>, HeadDims<32, 128>, HeadDims<32, 256>, HeadDims<64, 128>, HeadDims<64, 256>,
                               HeadDims<128, 256>>;
+// The non-causal kernels (attn_wgmma_bidir.cu) instantiate dqk == dv in {32, 64, 128} only.
+using BidirDims = HeadDimList<HeadDims<32, 32>, HeadDims<64, 64>, HeadDims<128, 128>>;
 template <int... DQK, int... DV>
 constexpr bool has_dims(HeadDimList<HeadDims<DQK, DV>...>, int dqk, int dv) { return ((dqk == DQK && dv == DV) || ...); }
 inline bool wgmma_dims(int dqk, int dv) { return has_dims(SquareDims{}, dqk, dv) || has_dims(MixedDims{}, dqk, dv); }
@@ -48,16 +50,13 @@ inline bool runs_on_fp16_operands(const hstu_attn_params& p) {
 constexpr bool fused_bwd_dims(int dqk, int dv) { return dqk == dv && (dqk == 64 || dqk == 128); }
 inline bool split_dq(const hstu_attn_params& p) { return !fused_bwd_dims(p.dqk, p.dv) || p.deterministic != 0; }
 
-// attn_wgmma_fwd.cu: whether the wgmma kernels take the call (dtype, dims, bias, views; sm_90) and the forward;
-// attn_wgmma_bwd.cu: the workspace and the backward
-bool wgmma_supported(const hstu_attn_params& p, bool bwd);
-size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd);
+// attn_wgmma_fwd.cu: whether the wgmma kernels take the call (dtype, dims, bias, views; sm_90; bidir: the non-causal mask,
+// BidirDims and no delta-q) and the forward; attn_wgmma_bwd.cu: the workspace and the backward
+bool wgmma_supported(const hstu_attn_params& p, bool bwd, bool bidir);
+size_t wgmma_workspace_bytes(const hstu_attn_params& p, bool bwd, bool bidir);
 int attn_wgmma_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bwd(const hstu_attn_params& p, cudaStream_t st);
-// attn_wgmma_bidir.cu: the non-causal mask at dqk == dv in {32, 64, 128}, no delta-q; wgmma_supported otherwise.  Its
-// workspace (the scaled fp16 operands of bf16 at d = 32, or 0), its forward and its (split) backward
-bool wgmma_bidir_supported(const hstu_attn_params& p, bool bwd);
-size_t wgmma_bidir_workspace_bytes(const hstu_attn_params& p, bool bwd);
+// attn_wgmma_bidir.cu: the non-causal forward and its (split) backward
 int attn_wgmma_bidir_fwd(const hstu_attn_params& p, cudaStream_t st);
 int attn_wgmma_bidir_bwd(const hstu_attn_params& p, cudaStream_t st);
 // attn_wgmma_bwd.cu: the bf16 d = 32 backward on the fp16 operands a forward kept (hstu_attn_bwd_on_fp16_operands)

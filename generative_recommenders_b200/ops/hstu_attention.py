@@ -16,6 +16,8 @@ import torch
 from .. import _lib
 from ..common import HammerKernel, require_cuda_kernel, switch_to_contiguous_if_needed
 
+_FP8 = torch.float8_e4m3fn
+
 
 def _fill_common(p, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
                  min_full_attn_seq_len, impl, delta_q_len=0):
@@ -47,16 +49,39 @@ def _fill_common(p, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_a
     p.v_row_stride, p.v_head_stride = v.stride(0), v.stride(1)
 
 
+def _aligned_buffer(nbytes: int, device):
+    """(buffer, base): a uint8 tensor holding nbytes from a 256-byte aligned base address, as the library's workspaces and
+    kept operands need; (None, None) for 0 bytes."""
+    if nbytes == 0:
+        return None, None
+    buf = torch.empty(nbytes + 256, dtype=torch.uint8, device=device)
+    return buf, (buf.data_ptr() + 255) // 256 * 256
+
+
 def _workspace(p, bwd: bool, device, causal: bool = True):
     size = _lib.lib().hstu_attn_workspace_bytes if causal else _lib.lib().hstu_attn_bidir_workspace_bytes
-    nbytes = size(C.byref(p), int(bwd))
-    if nbytes == 0:
-        p.workspace, p.workspace_bytes = None, 0
-        return None
-    ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=device)
-    base = (ws.data_ptr() + 255) // 256 * 256
-    p.workspace, p.workspace_bytes = base, nbytes
+    p.workspace_bytes = size(C.byref(p), int(bwd))
+    ws, p.workspace = _aligned_buffer(p.workspace_bytes, device)
     return ws
+
+
+def _fwd_params(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
+                min_full_attn_seq_len, impl, delta_q_len, out, out_dtype):
+    """(p, out, device) of a forward: q, k, v, seq_offsets, num_targets on one CUDA device and contiguous where the kernels
+    need it, and out, allocated [rows of q, H, dv] in out_dtype if None."""
+    dev = _lib.require_cuda(q, k, v, seq_offsets, num_targets)
+    q, k, v = _prep(q, k, v)
+    seq_offsets = seq_offsets.contiguous()
+    if num_targets is not None:
+        num_targets = num_targets.contiguous()
+    if out is None:
+        out = torch.empty((q.shape[0], q.shape[1], v.shape[2]), dtype=out_dtype, device=dev)
+    p = _lib.AttnParams()
+    _fill_common(p, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
+                 min_full_attn_seq_len, impl, delta_q_len)
+    p.out = out.data_ptr()
+    p.o_row_stride, p.o_head_stride = out.stride(0), out.stride(1)
+    return p, out, dev
 
 
 def _prep(*ts):
@@ -110,23 +135,12 @@ def cuda_hstu_attention_fwd(
             raise RuntimeError("fp8 attention: the relative bias and delta_q are not supported")
         return cuda_hstu_attention_fwd_fp8(max_seq_len, alpha, q, k, v, seq_offsets, descales, num_targets, max_attn_len,
                                            contextual_seq_len, min_full_attn_seq_len, impl, out)
-    dev = _lib.require_cuda(q, k, v, seq_offsets, num_targets)
-    q, k, v = _prep(q, k, v)
-    seq_offsets = seq_offsets.contiguous()
-    if num_targets is not None:
-        num_targets = num_targets.contiguous()
-    if out is None:
-        out = torch.empty((q.shape[0], q.shape[1], v.shape[2]), dtype=v.dtype, device=dev)
-    p = _lib.AttnParams()
-    _fill_common(p, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
-                 min_full_attn_seq_len, impl, delta_q_len)
-    p.out = out.data_ptr()
-    p.o_row_stride, p.o_head_stride = out.stride(0), out.stride(1)
+    p, out, dev = _fwd_params(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
+                              min_full_attn_seq_len, impl, delta_q_len, out, v.dtype)
     keep = _fill_bias(p, bias, None)
     kept = _lib.lib().hstu_attn_fp16_operands_bytes(C.byref(p)) if fp16_operands is not None else 0
     if kept:
-        fp16_operands.buf = torch.empty(kept + 256, dtype=torch.uint8, device=dev)
-        fp16_operands.base = (fp16_operands.buf.data_ptr() + 255) // 256 * 256
+        fp16_operands.buf, fp16_operands.base = _aligned_buffer(kept, dev)
         fp16_operands.nbytes = kept
         ws = None  # the pre-pass writes into the operands buffer instead of a workspace
         with torch.cuda.device(dev), _lib.timed("attn_fwd", dev):
@@ -134,18 +148,15 @@ def cuda_hstu_attention_fwd(
                        "hstu_attn_fwd_keep_fp16_operands")
     else:
         ws = _workspace(p, False, dev) if causal else _workspace(p, False, dev, causal=False)
-        name = "hstu_attn_fwd" if causal else "hstu_attn_fwd_bidir"
-        with torch.cuda.device(dev), _lib.timed(name[len("hstu_"):], dev):
-            _lib.check(getattr(_lib.lib(), name)(C.byref(p), _lib.stream_ptr(dev)), name)
+        run, name = (_lib.lib().hstu_attn_fwd, "attn_fwd") if causal else (_lib.lib().hstu_attn_fwd_bidir, "attn_fwd_bidir")
+        with torch.cuda.device(dev), _lib.timed(name, dev):
+            _lib.check(run(C.byref(p), _lib.stream_ptr(dev)), run.__name__)
     if delta_q_len:  # a workspace holds the partials of split key chunks: the attention kernel, then their reduction
         _lib.note_launch(2 if ws is not None else 1)
     else:  # bf16 at d = 32: amax and convert kernels before the attention kernel (into the workspace or the operands buffer)
         _lib.note_launch(3 if ws is not None or kept else 1)
     del ws, keep
     return out
-
-
-_FP8 = torch.float8_e4m3fn
 
 
 def _refuse_bidir(q, k, v, delta_q_len=0, bias=None, descales=None):
@@ -171,33 +182,13 @@ def cuda_hstu_attention_fwd_fp8(
     if not all(t.dtype == _FP8 for t in (q, k, v)):
         raise RuntimeError(f"fp8 attention: q, k and v must all be torch.float8_e4m3fn (got {q.dtype}, {k.dtype}, {v.dtype}); "
                            "descales apply to fp8 inputs only")
-    dev = _lib.require_cuda(q, k, v, seq_offsets, num_targets)
-    q, k, v = _prep(q, k, v)
-    seq_offsets = seq_offsets.contiguous()
-    if num_targets is not None:
-        num_targets = num_targets.contiguous()
-    B, H = seq_offsets.numel() - 1, q.shape[1]
-    ds = _lib.Descales()
-    for name, d in zip("qkv", descales if descales is not None else (None, None, None)):
-        if d is None:
-            continue
-        if d.dtype != torch.float32 or tuple(d.shape) != (B, H):
-            raise RuntimeError(f"fp8 attention: {name}_descale must be an fp32 [B, H] = [{B}, {H}] tensor "
-                               f"(got {d.dtype} {tuple(d.shape)})")
-        if d.device != dev:
-            raise RuntimeError(f"fp8 attention: {name}_descale is on {d.device}, the inputs on {dev}")
-        setattr(ds, name, d.data_ptr())
-        setattr(ds, f"{name}_batch_stride", d.stride(0))
-        setattr(ds, f"{name}_head_stride", d.stride(1))
-    if out is None:
-        out = torch.empty((q.shape[0], H, v.shape[2]), dtype=torch.bfloat16, device=dev)
-    elif out.dtype != torch.bfloat16:
+    if out is not None and out.dtype != torch.bfloat16:
         raise RuntimeError(f"fp8 attention: out must be bf16 (got {out.dtype})")
-    p = _lib.AttnParams()
-    _fill_common(p, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
-                 min_full_attn_seq_len, impl)
-    p.out = out.data_ptr()
-    p.o_row_stride, p.o_head_stride = out.stride(0), out.stride(1)
+    p, out, dev = _fwd_params(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
+                              min_full_attn_seq_len, impl, 0, out, torch.bfloat16)
+    ds = _lib.Descales()
+    _fill_descales(ds, "qkv", descales if descales is not None else (None, None, None), p.batch, p.heads, dev,
+                   "fp8 attention")
     ws = _workspace(p, False, dev)
     with torch.cuda.device(dev), _lib.timed("attn_fwd_fp8", dev):
         _lib.check(_lib.lib().hstu_attn_fwd_fp8(C.byref(p), C.byref(ds), _lib.stream_ptr(dev)), "hstu_attn_fwd_fp8")
@@ -239,28 +230,14 @@ def cuda_hstu_attention_fwd_delta_fp8_kv(
         raise RuntimeError(f"{what}: delta_q_len must be > 0 (got {delta_q_len})")
     if impl == _lib.IMPL_GENERIC:
         raise RuntimeError(f"{what}: runs on the wgmma kernels only (the generic kernels take no fp8 input)")
-    dev = _lib.require_cuda(delta_q, k, v, seq_offsets, num_targets)
-    delta_q, k, v = _prep(delta_q, k, v)
-    seq_offsets = seq_offsets.contiguous()
-    if num_targets is not None:
-        num_targets = num_targets.contiguous()
-    B, H = seq_offsets.numel() - 1, delta_q.shape[1]
-    ds = _lib.Descales()
-    _fill_descales(ds, "kv", kv_descales if kv_descales is not None else (None, None), B, H, dev, what)
-    if out is None:
-        out = torch.empty((delta_q.shape[0], H, v.shape[2]), dtype=delta_q.dtype, device=dev)
-    elif out.dtype != delta_q.dtype:
+    if out is not None and out.dtype != delta_q.dtype:
         raise RuntimeError(f"{what}: out must have the dtype of delta_q ({delta_q.dtype}, got {out.dtype})")
-    p = _lib.AttnParams()
-    _fill_common(p, max_seq_len, alpha, delta_q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
-                 min_full_attn_seq_len, impl, delta_q_len)
-    p.out = out.data_ptr()
-    p.o_row_stride, p.o_head_stride = out.stride(0), out.stride(1)
-    nbytes = _lib.lib().hstu_attn_fp8_kv_workspace_bytes(C.byref(p))
-    ws = None
-    if nbytes:
-        ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
-        p.workspace, p.workspace_bytes = (ws.data_ptr() + 255) // 256 * 256, nbytes
+    p, out, dev = _fwd_params(max_seq_len, alpha, delta_q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
+                              min_full_attn_seq_len, impl, delta_q_len, out, delta_q.dtype)
+    ds = _lib.Descales()
+    _fill_descales(ds, "kv", kv_descales if kv_descales is not None else (None, None), p.batch, p.heads, dev, what)
+    p.workspace_bytes = _lib.lib().hstu_attn_fp8_kv_workspace_bytes(C.byref(p))
+    ws, p.workspace = _aligned_buffer(p.workspace_bytes, dev)
     with torch.cuda.device(dev), _lib.timed("attn_fwd_delta_fp8_kv", dev):
         _lib.check(_lib.lib().hstu_attn_fwd_delta_fp8_kv(C.byref(p), C.byref(ds), _lib.stream_ptr(dev)),
                    "hstu_attn_fwd_delta_fp8_kv")
@@ -325,9 +302,8 @@ def cuda_hstu_attention_bwd(
     keep = _fill_bias(p, bias, dbias)
     if kept:  # the amax and convert kernels over dO alone, then the dK/dV and dQ kernels
         p.q = p.k = p.v = None
-        nbytes = _lib.lib().hstu_attn_bwd_fp16_operands_workspace_bytes(C.byref(p))
-        ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
-        p.workspace, p.workspace_bytes = (ws.data_ptr() + 255) // 256 * 256, nbytes
+        p.workspace_bytes = _lib.lib().hstu_attn_bwd_fp16_operands_workspace_bytes(C.byref(p))
+        ws, p.workspace = _aligned_buffer(p.workspace_bytes, dev)
         with torch.cuda.device(dev), _lib.timed("attn_bwd", dev):
             _lib.check(_lib.lib().hstu_attn_bwd_on_fp16_operands(C.byref(p), fp16_operands.base, fp16_operands.nbytes,
                                                                  _lib.stream_ptr(dev)), "hstu_attn_bwd_on_fp16_operands")
@@ -338,9 +314,9 @@ def cuda_hstu_attention_bwd(
         del ws, keep
         return
     ws = _workspace(p, True, dev) if causal else _workspace(p, True, dev, causal=False)
-    name = "hstu_attn_bwd" if causal else "hstu_attn_bwd_bidir"
-    with torch.cuda.device(dev), _lib.timed(name[len("hstu_"):], dev):
-        _lib.check(getattr(_lib.lib(), name)(C.byref(p), _lib.stream_ptr(dev)), name)
+    run, name = (_lib.lib().hstu_attn_bwd, "attn_bwd") if causal else (_lib.lib().hstu_attn_bwd_bidir, "attn_bwd_bidir")
+    with torch.cuda.device(dev), _lib.timed(name, dev):
+        _lib.check(run(C.byref(p), _lib.stream_ptr(dev)), run.__name__)
     # wgmma path: dK/dV kernel + dQ kernel (d = 32, after the amax and convert kernels for bf16; deterministic d = 64 / 128
     # and every non-causal call: no workspace, no memset, no convert) or main kernel + dQ convert; generic path: dK/dV
     # kernel + dQ kernel
@@ -382,27 +358,30 @@ def _fill_bias(p, bias, dbias):
 
 
 class _HSTUAttentionFunction(torch.autograd.Function):
+    """The autograd of hstu_mha and torch.ops.hstu.hstu_mha.  deterministic: that of cuda_hstu_attention_bwd (None follows
+    torch.are_deterministic_algorithms_enabled() when the backward runs)."""
+
     @staticmethod
     def forward(ctx, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, contextual_seq_len,
-                min_full_attn_seq_len, impl, causal=True):
+                min_full_attn_seq_len, impl, causal, deterministic):
         # no Fp16Operands here: q, k, v are saved anyway, so the copies would double the saved bytes to spare only the
         # backward's pre-pass over q, k, v
         out = cuda_hstu_attention_fwd(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
                                       contextual_seq_len, min_full_attn_seq_len, impl, causal=causal)
         ctx.save_for_backward(q, k, v, seq_offsets, num_targets)
-        ctx.args = (max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full_attn_seq_len, impl, causal)
+        ctx.args = (max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full_attn_seq_len, impl, causal, deterministic)
         return out
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, seq_offsets, num_targets = ctx.saved_tensors
-        max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full, impl, causal = ctx.args
+        max_seq_len, alpha, max_attn_len, contextual_seq_len, min_full, impl, causal, deterministic = ctx.args
         dq = torch.empty(q.shape, dtype=q.dtype, device=q.device)
         dk = torch.empty(k.shape, dtype=k.dtype, device=k.device)
         dv = torch.empty(v.shape, dtype=v.dtype, device=v.device)
         cuda_hstu_attention_bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, num_targets, max_attn_len,
-                                contextual_seq_len, min_full, impl, causal=causal)
-        return None, None, dq, dk, dv, None, None, None, None, None, None, None
+                                contextual_seq_len, min_full, impl, deterministic=deterministic, causal=causal)
+        return None, None, dq, dk, dv, None, None, None, None, None, None, None, None
 
 
 def hstu_mha(
@@ -441,7 +420,7 @@ def hstu_mha(
     require_cuda_kernel(kernel, "hstu_mha")
     torch._assert(dropout_pr < 1e-6, "dropout for the CUDA path is not implemented")
     return _HSTUAttentionFunction.apply(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
-                                        contextual_seq_len, min_full_attn_seq_len, impl, bool(causal))
+                                        contextual_seq_len, min_full_attn_seq_len, impl, bool(causal), None)
 
 
 def delta_hstu_mha(

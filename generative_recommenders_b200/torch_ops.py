@@ -25,7 +25,8 @@ from typing import List, Optional
 
 import torch
 
-from .ops.hstu_attention import cuda_hstu_attention_bwd, cuda_hstu_attention_fwd
+from . import _lib
+from .ops.hstu_attention import _FP8, _HSTUAttentionFunction, cuda_hstu_attention_bwd, cuda_hstu_attention_fwd
 
 _LIB = None
 
@@ -38,9 +39,6 @@ _FWD = ("hstu_mha_fwd(SymInt max_seq_len, float alpha, Tensor q, Tensor k, Tenso
 _BWD = ("hstu_mha_bwd(int max_seq_len, float alpha, Tensor dout, Tensor q, Tensor k, Tensor v, Tensor dq, Tensor dk, Tensor dv, "
         "Tensor? seq_offsets, bool causal, Tensor? num_targets, Tensor? attn_scale, int max_attn_len, int min_full_attn_seq_len, "
         "int contextual_seq_len, bool sort_by_length, bool deterministic, int sm_margin) -> Tensor[]")
-
-
-_FP8 = torch.float8_e4m3fn
 
 
 def _check(causal, seq_offsets, attn_scale, descales, qkv=()):
@@ -76,26 +74,6 @@ def _deterministic(flag):
     return True if flag else None
 
 
-class _Mha(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, min_full, ctx_len, deterministic,
-                causal=True):
-        out = cuda_hstu_attention_fwd(max_seq_len, alpha, q, k, v, seq_offsets, num_targets, max_attn_len, ctx_len, min_full,
-                                      causal=causal)
-        ctx.save_for_backward(q, k, v, seq_offsets, num_targets)
-        ctx.cfg = (max_seq_len, alpha, max_attn_len, min_full, ctx_len, deterministic, causal)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        q, k, v, seq_offsets, num_targets = ctx.saved_tensors
-        max_seq_len, alpha, max_attn_len, min_full, ctx_len, deterministic, causal = ctx.cfg
-        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        cuda_hstu_attention_bwd(max_seq_len, alpha, dout, q, k, v, dq, dk, dv, seq_offsets, num_targets, max_attn_len, ctx_len,
-                                min_full, deterministic=_deterministic(deterministic), causal=causal)
-        return None, None, dq, dk, dv, None, None, None, None, None, None, None
-
-
 def _mha(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_scale, max_attn_len, min_full_attn_seq_len,
          contextual_seq_len, q_descale, k_descale, v_descale, sort_by_length, deterministic, sm_margin):
     descales = (q_descale, k_descale, v_descale)
@@ -106,8 +84,9 @@ def _mha(max_seq_len, alpha, q, k, v, seq_offsets, causal, num_targets, attn_sca
                                "run it under torch.no_grad() or on tensors that do not require grad")
         return cuda_hstu_attention_fwd(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
                                        contextual_seq_len, min_full_attn_seq_len, descales=descales, causal=bool(causal))
-    return _Mha.apply(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len, min_full_attn_seq_len,
-                      contextual_seq_len, bool(deterministic), bool(causal))
+    return _HSTUAttentionFunction.apply(int(max_seq_len), alpha, q, k, v, seq_offsets, num_targets, max_attn_len,
+                                        contextual_seq_len, min_full_attn_seq_len, _lib.IMPL_AUTO, bool(causal),
+                                        _deterministic(deterministic))
 
 
 def _fwd_meta(max_seq_len, alpha, q, k, v, *args):
@@ -124,7 +103,7 @@ def register() -> None:
     lib.define(_MHA)
     lib.define(_FWD)
     lib.define(_BWD)
-    lib.impl("hstu_mha", _mha, "CompositeImplicitAutograd")  # autograd through _Mha; fwd / bwd below are the raw kernels
+    lib.impl("hstu_mha", _mha, "CompositeImplicitAutograd")  # autograd through _HSTUAttentionFunction; fwd / bwd: raw kernels
     lib.impl("hstu_mha_fwd", _fwd, "CUDA")
     lib.impl("hstu_mha_bwd", _bwd, "CUDA")
     lib.impl("hstu_mha_fwd", _fwd_meta, "Meta")

@@ -205,3 +205,62 @@ def test_c_abi_refusals_and_routing(lib):
         assert lib.hstu_attn_bidir_select_impl(C.byref(params(impl=_lib.IMPL_UMMA, **kw)), 0) == -2
         assert b"generic" in lib.hstu_last_error()
     assert lib.hstu_attn_bidir_workspace_bytes(C.byref(params()), 1) == 0  # empty problem
+
+
+DEVICE_PTR = b"expected a CUDA device pointer"
+# (case, backward, expected return of hstu_attn_{fwd|bwd}, hstu_attn_{fwd|bwd}_bidir, hstu_attn_select_impl,
+# hstu_attn_bidir_select_impl, hstu_attn_workspace_bytes, hstu_attn_bidir_workspace_bytes); a refusal is (code, message part).
+# The entries differ where the table says so: the causal ones refuse e4m3 themselves, return 0 on an empty problem and bind
+# the device of q before routing; the non-causal ones route first.
+ENTRY_TABLE = [
+    (dict(rows=0), False, 0, 0, 1, 1, 0, 0),
+    (dict(rows=0), True, 0, 0, 1, 1, 0, 0),
+    (dict(rows=0, dtype="e4m3"), False, (-1, b"go through hstu_attn_fwd_fp8"), (-2, b"fp8 (e4m3) inputs are not supported"),
+     (-2, b"the generic kernels take no fp8 input"), (-2, b"fp8 (e4m3) inputs are not supported"), 0, 0),
+    (dict(rows=0, dtype="e4m3"), True, (-2, b"hstu_attn_bwd: fp8 (e4m3) attention has no backward"),
+     (-2, b"fp8 (e4m3) inputs are not supported"), (-2, b"fp8 (e4m3) attention has no backward: hstu_attn_fwd_fp8"),
+     (-2, b"fp8 (e4m3) inputs are not supported"), 0, 0),
+    (dict(rows=0, delta=4), False, 0, (-2, b"delta_q (the KV-cached forward) is causal only"), 1,
+     (-2, b"delta_q (the KV-cached forward) is causal only"), 0, 0),
+    (dict(rows=0, bias=True), True, 0, (-2, b"the relative bias is not supported"),
+     (-2, b"deterministic backward with a relative bias"), (-2, b"the relative bias is not supported"), 0, 0),
+    (dict(dqk=48, impl=2), False, (-1, DEVICE_PTR), (-2, b"it takes bf16 / fp16 at dqk == dv in {32, 64, 128}"),
+     (-2, b"delta=0 bias=0"), (-2, b"non-causal wgmma path does not support this problem (dtype=1 dqk=48 dv=48)"), 0, 0),
+    (dict(dqk=48, impl=2), True, (-1, DEVICE_PTR), (-2, b"non-causal wgmma path"), (-2, b"delta=0 bias=0"),
+     (-2, b"non-causal wgmma path"), 0, 0),
+    (dict(), True, (-1, DEVICE_PTR), (-1, DEVICE_PTR), 1, 1, 0, 0),
+    (dict(dtype="e4m3", impl=0), False, (-1, b"go through hstu_attn_fwd_fp8"), (-2, b"fp8 (e4m3) inputs are not supported"),
+     2, (-2, b"fp8 (e4m3) inputs are not supported"), 4096 * 2 * 32 * 2, 0),
+    (dict(delta=4), True, *[(-1, b"backward of delta-q attention is not defined")] * 4, 0, 0),
+    (None, False, *[(-1, b"params is NULL")] * 4, 0, 0),
+]
+
+
+@pytest.mark.parametrize("case,bwd,want", [(c, b, tuple(w)) for c, b, *w in ENTRY_TABLE])
+def test_c_abi_attention_entries_at_both_masks(lib, case, bwd, want):
+    """Return code and message of every attention entry, causal and non-causal, for refused and empty problems, with
+    placeholder pointers: nothing here needs a device.  Problems the argument checks pass reach the device binding of the
+    run entries, which refuses a placeholder q on any machine.  Default impl: generic, which routes without a device query."""
+    from generative_recommenders_b200 import _lib
+    from test_attention_deterministic_cpu import _params
+
+    p = None
+    if case is not None:
+        kw = dict(case)
+        dtype = {"bf16": _lib.BF16, "e4m3": _lib.E4M3}[kw.pop("dtype", "bf16")]
+        dqk = kw.pop("dqk", 32)
+        p = _params(dtype, dqk, deterministic=1, impl=kw.pop("impl", _lib.IMPL_GENERIC), rows=kw.pop("rows", 4096),
+                    bias=kw.pop("bias", False))
+        p.delta_q_len = kw.pop("delta", 0)
+        assert not kw, kw
+        p = C.byref(p)
+    d = "bwd" if bwd else "fwd"
+    calls = ((f"hstu_attn_{d}", None), (f"hstu_attn_{d}_bidir", None), ("hstu_attn_select_impl", int(bwd)),
+             ("hstu_attn_bidir_select_impl", int(bwd)), ("hstu_attn_workspace_bytes", int(bwd)),
+             ("hstu_attn_bidir_workspace_bytes", int(bwd)))
+    for (name, arg), w in zip(calls, want):
+        rc = getattr(lib, name)(p, arg)
+        if isinstance(w, tuple):
+            assert (rc, w[1] in lib.hstu_last_error()) == (w[0], True), (name, rc, lib.hstu_last_error(), w)
+        else:
+            assert rc == w, (name, rc, lib.hstu_last_error(), w)

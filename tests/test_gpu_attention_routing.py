@@ -1,6 +1,7 @@
 """The routing table of the attention C ABI on an sm_90 device: for every (dtype, dqk, dv) the wgmma kernels take, and a few
-they refuse, what hstu_attn_select_impl, hstu_attn_workspace_bytes, hstu_attn_fp16_operands_bytes and
-hstu_attn_bwd_fp16_operands_workspace_bytes return, forward and backward, with delta-q (one key chunk and several), the
+they refuse, what hstu_attn_select_impl, hstu_attn_workspace_bytes, hstu_attn_fp16_operands_bytes,
+hstu_attn_bwd_fp16_operands_workspace_bytes and the non-causal hstu_attn_bidir_select_impl and
+hstu_attn_bidir_workspace_bytes return, forward and backward, with delta-q (one key chunk and several), the
 deterministic flag, a relative bias, each impl request, and one misaligned view per tensor.  Nothing is launched: the
 pointers are placeholders.  `_want` is the table; a routing change edits it on purpose."""
 import ctypes as C
@@ -67,8 +68,24 @@ def _select(dtype, dqk, dv, bwd, det=0, bias=False, batch=2, delta=0, mis=None, 
     return _lib.IMPL_UMMA if can else _lib.IMPL_GENERIC
 
 
+def _select_bidir(dtype, dqk, dv, bwd, det=0, bias=False, batch=2, delta=0, mis=None, impl=0):
+    """hstu_attn_bidir_select_impl as the table has it: the non-causal wgmma kernels take bf16 / fp16 at dqk == dv in
+    {32, 64, 128} without delta-q, and the wgmma views of the causal ones."""
+    from generative_recommenders_b200 import _lib
+
+    if delta or bias or dtype == _lib.E4M3:  # refused whatever impl asks
+        return HSTU_ERR_UNSUPPORTED
+    can = dtype in (_lib.BF16, _lib.F16) and dqk == dv and dqk in (32, 64, 128) and mis not in READS[bwd]
+    if impl == _lib.IMPL_GENERIC:
+        return _lib.IMPL_GENERIC
+    if impl == _lib.IMPL_UMMA:
+        return _lib.IMPL_UMMA if can else HSTU_ERR_UNSUPPORTED
+    return _lib.IMPL_UMMA if can else _lib.IMPL_GENERIC
+
+
 def _want(dtype, dqk, dv, bwd, **v):
-    """(select_impl, workspace_bytes, fp16_operands_bytes, bwd_fp16_operands_workspace_bytes)"""
+    """(select_impl, workspace_bytes, fp16_operands_bytes, bwd_fp16_operands_workspace_bytes, bidir_select_impl,
+    bidir_workspace_bytes)"""
     from generative_recommenders_b200 import _lib
 
     batch, delta, det = v.get("batch", 2), v.get("delta", 0), v.get("det", 0)
@@ -89,7 +106,10 @@ def _want(dtype, dqk, dv, bwd, **v):
         ws = ROWS * H * dqk * 4  # the fused backward's fp32 dQ accumulator
     fwd_sel = _select(dtype, dqk, dv, False, **v)
     kept = amax + 3 * copy if dtype == _lib.BF16 and dqk == dv == 32 and not delta and fwd_sel == _lib.IMPL_UMMA else 0
-    return sel, ws, kept, amax + copy
+    bidir_sel = _select_bidir(dtype, dqk, dv, bwd, **v)
+    # the non-causal backward is always split: its only workspace is the scaled fp16 operands of bf16 at d = 32
+    bidir_ws = amax + (4 if bwd else 3) * copy if bidir_sel == _lib.IMPL_UMMA and dtype == _lib.BF16 and dqk == 32 else 0
+    return sel, ws, kept, amax + copy, bidir_sel, bidir_ws
 
 
 def _dtypes():
@@ -120,7 +140,8 @@ def test_attention_routing_table(lib, dtype, dqk, dv):
             for impl in (_lib.IMPL_AUTO, _lib.IMPL_GENERIC, _lib.IMPL_UMMA):
                 p = C.byref(_case(code, dqk, dv, bwd, impl=impl, **v))
                 got = (lib.hstu_attn_select_impl(p, int(bwd)), lib.hstu_attn_workspace_bytes(p, int(bwd)),
-                       lib.hstu_attn_fp16_operands_bytes(p), lib.hstu_attn_bwd_fp16_operands_workspace_bytes(p))
+                       lib.hstu_attn_fp16_operands_bytes(p), lib.hstu_attn_bwd_fp16_operands_workspace_bytes(p),
+                       lib.hstu_attn_bidir_select_impl(p, int(bwd)), lib.hstu_attn_bidir_workspace_bytes(p, int(bwd)))
                 assert got == _want(code, dqk, dv, bwd, impl=impl, **v), (dtype, dqk, dv, "bwd" if bwd else "fwd", impl, v)
                 n += 1
     assert n == 3 * (15 + 13)
